@@ -1,14 +1,15 @@
 #!/usr/bin/env python
 """Benchmark of the so.infer() hot path (BASELINE.json metric: rows/s and output tok/s over a
-DataFrame column at 1/2/4/8 B200; % of roofline for the dominant kernels).
+DataFrame column at 1/2/4/8 H100; % of roofline for the dominant kernels).
 
     python bench.py --gpus 1 --steps 3 --warmup 3
+    python bench.py --gpus 1 --steps 1 --warmup 1 --dump-outputs DIR   # + the last step's outputs
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference            # CPU baseline arm
 
-Workload (config.workload): BASELINE.json configs[1] — ONE 20k-row synthetic product-review
-frame per step, qwen-3-4b architecture in bf16 (seeded random weights: no checkpoint exists
+Workload (config.workload): BASELINE.json configs[1] shape — ONE synthetic product-review frame
+(4,096 rows by default, --rows) per step, qwen-3-4b architecture in bf16 (seeded random weights: no checkpoint exists
 offline), system prompt + Sentiment enum output_schema, greedy.  The frame lives on rank 0.
 
 One "step" = one call of the public API on that frame, exactly what a user runs:
@@ -21,7 +22,7 @@ One "step" = one call of the public API on that frame, exactly what a user runs:
           HBM, NCCL broadcast, every rank selects its length-balanced share with a native
           kernel, runs it on its replica, NCCL gather on rank 0, ordered merge (results are
           positional, sutro/sdk.py:406-412), device -> host, write-back into the frame.
-          STRONG scaling: the same 20k rows at every N.
+          STRONG scaling: the same rows at every N.
 
 `e2e`    = rows/s of the K calls: barrier + synchronize on both sides, wall clock, host frame in,
            result column written back — host<->device copies inside.
@@ -79,31 +80,9 @@ def peaks():
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0,
-            "source": "fallback"}
-
-
-def ncu_traffic(csv_name: str, kernel: str):
-    """DRAM bytes (read + write) of one launch of `kernel` (substring of the kernel name) from a
-    committed `ncu --set full` capture under profiles/ (the per-launch summary
-    tools/profile_extract.py writes), or None.  The capture is of one representative launch of
-    the kernel class inside the same workload, not of this run."""
-    try:
-        import csv
-        with open(os.path.join(ROOT, "profiles", csv_name), newline="") as f:
-            rows = list(csv.reader(f))
-        hdr = rows[0]
-        scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-        cols = []
-        for i, h in enumerate(hdr):
-            if h.startswith(("dram_read", "dram_write")):
-                cols.append((i, scale[h[h.index("[") + 1:h.index("]")]]))
-        for r in rows[1:]:
-            if kernel in r[0]:
-                return sum(float(r[i]) * k for i, k in cols)
-        return None
-    except Exception:
-        return None
+    # NVIDIA's H100 SXM data sheet (700 W card; dense BF16): not reached, only the yardstick
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0,
+            "source": "data sheet (H100 SXM, 700 W)"}
 
 
 class ClockSampler:
@@ -131,6 +110,12 @@ class ClockSampler:
     def stop(self):
         if self.proc:
             self.proc.terminate()
+            try:
+                self.proc.wait(timeout=10)
+            except subprocess.TimeoutExpired:
+                self.proc.kill()
+                self.proc.wait()
+            self.proc = None
         sm = [float(r[0]) for r in self.rows if len(r) >= 7 and r[0].replace(".", "").isdigit()]
         if not sm:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["unavailable"]}
@@ -324,7 +309,7 @@ def run_reference_arm(args):
             "config": workload_config(args),
             "cpu_baseline": {"value": v, "unit": "rows/s", "cores": threads, "kind": "port",
                              "sample": f"{n_sample} rows per step x {args.steps} steps of the same "
-                                       "workload (a bounded sample of the 20k-row frame), CPU oracle "
+                                       "workload (a bounded sample of the frame), CPU oracle "
                                        "(oracle/model_ref.py); the reference repo has no local "
                                        "implementation of this path"},
             "e2e": {"value": v, "unit": "rows/s", "h2d_bytes_per_step": 0,
@@ -345,7 +330,7 @@ def workload_config(args, shape=None):
            "parallelism": f"one replica per GPU x{args.gpus}; the frame's rows are dealt to the "
                           "ranks by byte length (snake order), results gathered in row order on "
                           "rank 0",
-           "l2": "inputs_exceed_l2 (8 GB of weights + KV streamed per step; L2 is 126 MB)",
+           "l2": "inputs_exceed_l2 (8 GB of weights + KV streamed per step; L2 is 50 MB)",
            "max_slots": args.max_slots, "max_prefill_tokens": args.max_prefill_tokens,
            "decoding": "greedy + schema mask, jump-forward (forced JSON syntax is fed with the "
                        "prompt / appended, not decoded token by token)"}
@@ -428,7 +413,7 @@ def secondary_blocks(args, pk, dev, headline_eng, weights, vocab):
                    input_tokens_per_sec=r.stats["input_tokens"] / dt,
                    prompt_tokens_per_row_mean=r.stats["input_tokens"] / len(rows),
                    decode_steps=r.stats["decode_steps"], prefill_steps=r.stats["prefill_steps"],
-                   speed_of_light_rows_per_sec=267.0)
+                   speed_of_light_rows_per_sec=170.0)
         out["configs2_docs"] = blk
         log(f"secondary configs[2]: {blk['rows_per_sec']:.1f} rows/s, decode attention "
             f"{blk['attn_decode_gbs_non_shared_kv']:.0f} GB/s at {100 * blk['attn_decode_share_of_step']:.1f}% of the step")
@@ -516,6 +501,43 @@ def secondary_blocks(args, pk, dev, headline_eng, weights, vocab):
     return out
 
 
+# ----------------------------------------------------------------------------- outputs
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, outputs, job):
+    """What the timed call handed back to the caller in its last step, as .npy files:
+    outputs_utf8 (float32 [rows, max_bytes], UTF-8 bytes of each output string, -1 padded),
+    output_bytes (float64 [rows]), cum_logprobs (float32 [rows]) and, for schema jobs,
+    confidence (float64 [rows]).  When the strings would not fit the budget, a fixed seeded
+    sample of rows is written instead and its row indices go to sample_rows (float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    enc = [str(o).encode("utf-8") for o in outputs]
+    n = len(enc)
+    width = max((len(b) for b in enc), default=0)
+    per_row = 4 * width + 8 + 4 + 8
+    rows = np.arange(n)
+    if n and per_row * n > DUMP_LIMIT_BYTES - (1 << 20):
+        k = max(1, (DUMP_LIMIT_BYTES - (1 << 20)) // (per_row + 8))
+        rows = np.sort(np.random.default_rng(0).choice(n, size=k, replace=False))
+        np.save(os.path.join(out_dir, "sample_rows.npy"), rows.astype(np.float64))
+    text = np.full((len(rows), width), -1.0, dtype=np.float32)
+    for i, r in enumerate(rows):
+        b = np.frombuffer(enc[r], dtype=np.uint8)
+        text[i, :len(b)] = b
+    np.save(os.path.join(out_dir, "outputs_utf8.npy"), text)
+    np.save(os.path.join(out_dir, "output_bytes.npy"),
+            np.array([len(enc[r]) for r in rows], dtype=np.float64))
+    if job is not None and job.cum_logprobs is not None:
+        np.save(os.path.join(out_dir, "cum_logprobs.npy"),
+                np.asarray(job.cum_logprobs, dtype=np.float32)[rows])
+    if job is not None and getattr(job, "confidence", None) is not None:
+        np.save(os.path.join(out_dir, "confidence.npy"),
+                np.asarray(job.confidence, dtype=np.float64)[rows])
+    log(f"outputs of the last step written to {out_dir}")
+
+
 # ----------------------------------------------------------------------------- GPU arm
 def main():
     ap = argparse.ArgumentParser()
@@ -524,12 +546,15 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--model", default="qwen-3-4b")
-    ap.add_argument("--rows", type=int, default=20000, help="rows of the frame (whole job) per step")
+    # 4096 rows = 14 full 32k-token prefill steps per job: long enough to time the kernels at their
+    # production shapes, short enough that one H100 runs warm-up + timed steps in minutes (a
+    # 20,000-row frame takes 30-50 s per step there; --rows 20000 is the full configs[1] frame)
+    ap.add_argument("--rows", type=int, default=4096, help="rows of the frame (whole job) per step")
     ap.add_argument("--workload", default="sentiment", choices=["sentiment", "docs"],
                     help="sentiment = BASELINE.json configs[1] (the headline); docs = configs[2] "
                          "shape (~512-token prompts, 64 generated tokens, no schema)")
     ap.add_argument("--max-slots", type=int, default=3584,
-                    help="decode slots; 3584 = 14 x 256 rows quantises the CTA-pair GEMM tiles well")
+                    help="decode slots; 3584 = 28 x 128 rows fills whole 128-row GEMM tiles")
     ap.add_argument("--max-prefill-tokens", type=int, default=32768)
     ap.add_argument("--cpu-rows", type=int, default=8, help="max rows in the CPU-baseline sample")
     ap.add_argument("--cpu-budget-s", type=float, default=25.0,
@@ -537,12 +562,15 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true",
                     help="skip the configs[2]/[3]/[4] secondary blocks")
-    ap.add_argument("--docs-rows", type=int, default=2048)
-    ap.add_argument("--embed-rows", type=int, default=200000)
-    ap.add_argument("--extract-rows", type=int, default=1024)
+    # secondary samples sized so that the three blocks take about a minute on one H100
+    ap.add_argument("--docs-rows", type=int, default=1024)
+    ap.add_argument("--embed-rows", type=int, default=100000)
+    ap.add_argument("--extract-rows", type=int, default=512)
     ap.add_argument("--kv-pages", type=int, default=None,
-                    help="KV pool size in pages (default: 80%% of free memory); small pools keep "
-                         "ncu's save/restore cheap")
+                    help="KV pool size in pages (default: 80%% of free memory)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last step returned to the caller "
+                         "as DIR/<name>.npy (float32/float64, <= 64 MB in all)")
     args = ap.parse_args()
     global WORKLOAD
     WORKLOAD = args.workload
@@ -583,7 +611,9 @@ def main():
     vocab = VB.build_vocab(spec.family, spec.vocab_size, seed=0)
     eng = LocalEngine(spec, weights, vocab, device=dev, max_slots=args.max_slots,
                       max_prefill_tokens=args.max_prefill_tokens, kv_pages=args.kv_pages)
-    client = Sutro(verbose=False, cache_dir="/tmp/sb200-bench-cache")
+    import tempfile
+    cache_dir = tempfile.TemporaryDirectory(prefix="sb200-bench-cache-")   # removed at exit
+    client = Sutro(verbose=False, cache_dir=cache_dir.name)
     client.register_engine(args.model, eng)
     setup_s = time.perf_counter() - t0
     log(f"engine ready in {setup_s:.1f}s (kv_pages={eng.kv_pages})")
@@ -602,14 +632,18 @@ def main():
     log(f"{n_frames} frames of {args.rows} rows generated")
     kw = infer_kwargs(args.model)
 
+    last_job = None
+
     def step(i):
         """the user's call; returns the job's stats on rank 0"""
+        nonlocal last_job
         data = frames[i] if rank == 0 else []
         job_id = client.infer(data, **kw)
         if job_id is None:
             raise RuntimeError("infer() failed: " + str(
                 [j.failure_reason for j in client._jobs.values()][-1:]))
-        return client._jobs[job_id].stats
+        last_job = client._jobs[job_id]
+        return last_job.stats
 
     for i in range(args.warmup):
         t = time.perf_counter()
@@ -620,18 +654,22 @@ def main():
     clocks = ClockSampler(local)
     fence()
     clocks.start()
-    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    ev0.record()
-    t_start = time.perf_counter()
-    stats = []
-    for i in range(args.steps):
-        t = time.perf_counter()
-        stats.append(step(args.warmup + i))
-        log(f"step {i}: {time.perf_counter() - t:.2f}s")
-    ev1.record()
-    fence()
-    t_e2e = time.perf_counter() - t_start
-    clk = clocks.stop()
+    try:   # the sampler's nvidia-smi loop must end with the timed region, whatever happens in it
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record()
+        t_start = time.perf_counter()
+        stats = []
+        for i in range(args.steps):
+            t = time.perf_counter()
+            stats.append(step(args.warmup + i))
+            log(f"step {i}: {time.perf_counter() - t:.2f}s")
+        ev1.record()
+        fence()
+        t_e2e = time.perf_counter() - t_start
+    finally:
+        clk = clocks.stop()
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, list(frames[-1]["inference_result"]), last_job)
 
     # ---- counters: rank 0 holds the job-wide numbers (sharded stats are already aggregated) ----
     tt = torch.tensor([t_e2e], dtype=torch.float64, device=dev)
@@ -668,17 +706,11 @@ def main():
         prof["_kv_bytes_per_token"] = spec.kv_bytes_per_token
         kb = kernel_block(prof, pk, prof.get("prefix_cached_tokens", 0))
         kms = prof["kernel_ms"]
-        roofline = {"kernel": "gemm_bf16_tn_kernel / gemm2_bf16_tn_kernel (tcgen05)",
+        roofline = {"kernel": "gemm_bf16_tn_kernel (wgmma)",
                     "bound": "tensor", "achieved": kb["gemm_tflops"],
                     "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s",
                     "frac": kb["gemm_frac_of_sustained_peak"],
-                    "traffic": ncu_traffic("r02_ncu_prefill_step.csv", "gemm2_bf16_tn_kernel<2, 7"),
-                    "traffic_note": "bytes of ONE gate/up GEMM launch of a full prefill step "
-                                    "(M=32670, N=19456, K=2560; algorithmic 903 MB = A 167 + "
-                                    "W 100 + SwiGLU output 636; W does not fit L2, so A and W "
-                                    "are re-read) from the committed capture "
-                                    "profiles/r02_ncu_prefill_step.csv, not from this run",
-                    "peak_source": pk["source"] + " (sustained: kernel timed inside a long step)",
+                    "peak_source": pk["source"],
                     "share_of_step": kb["share"]["gemm"],
                     "launches": prof["kernel_launches"]["gemm"],
                     "avg_launch_ms": kms["gemm"] / max(1, prof["kernel_launches"]["gemm"]),
@@ -687,7 +719,6 @@ def main():
                          "achieved": kb["attn_decode_gbs_non_shared_kv"], "peak": pk["hbm_gbs"],
                          "unit": "GB/s", "frac": kb["attn_decode_frac_of_hbm_peak"],
                          "bytes": "non-shared KV only (the shared system-prompt pages are L2 hits)",
-                         "traffic": ncu_traffic("r02_ncu_decode_side.csv", "attn_decode_warp_kernel"),
                          "share_of_step": kb["attn_decode_share_of_step"],
                          "launches": prof["kernel_launches"]["attn_decode"],
                          "note": "the headline job barely decodes (jump-forward); the graded "

@@ -1,4 +1,4 @@
-/* sutro_b200 — C-ABI of the B200-native local backend for sutro.infer().
+/* sutro_b200 — C-ABI of the H100-native local backend for sutro.infer().
  *
  * The reference SDK (sutro-sh/sutro) has no FFI: Sutro.infer() serialises the
  * column and POSTs it to a hosted service (sutro/sdk.py:195-223).  This header
@@ -44,8 +44,9 @@ int sb200_device_info(int* sm_count, int* cc_major, int* cc_minor, size_t* total
 #define SB200_EPI_SWIGLU_BF16 2   /* D[:,j] = silu(acc[:,2j]) * acc[:,2j+1]       */
 #define SB200_EPI_STORE_F32 3     /* D = A W^T in fp32 (logits)                   */
 
-/* K1: D[M,N] = A[M,K] W[N,K]^T on tcgen05 tensor cores.  A may be the head of a
- * larger buffer with a_rows >= M rows.  block_n: 0 = auto, else 64/128/256. */
+/* K1: D[M,N] = A[M,K] W[N,K]^T on wgmma tensor cores.  A may be the head of a
+ * larger buffer with a_rows >= M rows.  block_n: 0 = auto, else 64/128/256; 512 is accepted for
+ * callers of the first ABI version and runs the 256-wide tile. */
 int sb200_gemm_bf16_tn(const void* a, int a_rows, const void* w, void* d, const void* resid, int M,
                        int N, int K, int ldd, int epilogue, int block_n, void* stream);
 
@@ -89,12 +90,14 @@ int sb200_attn_prefill(const void* qkv, void* out, const void* kv_layer, const i
                        const int32_t* seq_past, int hq, int hkv, float scale, void* stream);
 int sb200_attn_prefill_q_tile(int hq, int hkv);
 
-/* K3 on tcgen05 tensor cores (the engine's prefill path): causal varlen attention over DENSE
+/* K3 on wgmma tensor cores (the engine's prefill path): causal varlen attention over DENSE
  * K/V.  qkv:[t_rows, (hq+2*hkv)*128] holds q AND the post-norm/RoPE k, v of the new tokens
  * (what sb200_gemm_qkv_rope leaves there); prefix_kv:[n_layers, prefix_rows, 2*hkv*128]
  * (K heads | V heads) holds the shared prefix, NULL when no sequence has a past.
  * items:[n_items] {seq, q_tile_start}; sequence i attends to prefix rows [0, seq_past[i])
- * and to its own rows [seq_q_start[i], +seq_q_len[i]) causally. */
+ * and to its own rows [seq_q_start[i], +seq_q_len[i]) causally.  K/V are read in 32-row boxes:
+ * the k/v values of the rows up to 31 past a sequence's last token (in qkv and in prefix_kv)
+ * must be finite, or that sequence's output is NaN. */
 int sb200_attn_prefill_dense(const void* qkv, int t_rows, void* out, const void* prefix_kv,
                              int prefix_rows, int n_layers, int layer, const int32_t* items,
                              int n_items, const int32_t* seq_q_start, const int32_t* seq_q_len,

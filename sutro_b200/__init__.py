@@ -1,4 +1,4 @@
-"""sutro_b200 — B200-native local backend for the sutro.infer() hot path.
+"""sutro_b200 — H100-native local backend for the sutro.infer() hot path.
 
     import sutro_b200 as so
     job_id = so.infer(df, column="review", model="qwen-3-4b",

@@ -9,7 +9,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# SB200_LIB: load another build of the same library (tools/build_trace_lib.sh's instrumented twin)
+# SB200_LIB: load another build of the same library (e.g. one compiled with different flags)
 LIB_PATH = os.environ.get("SB200_LIB") or os.path.join(_HERE, "libsutro_b200.so")
 
 _lib = None

@@ -1,30 +1,36 @@
-// sutro_b200 — K3 (tensor-core path): causal varlen prefill attention on tcgen05.
+// sutro_b200 — K3 (tensor-core path): causal varlen prefill attention on Hopper wgmma.
 //
 // The engine never splits a row's prompt over prefill steps, so a new token attends to
 // [shared prefix | the row's own new tokens].  Both live in DENSE row-major buffers here:
-// the fused QKV epilogue (gemm_tcgen05.cu) leaves post-norm / post-RoPE K and V in the qkv
+// the fused QKV epilogue (gemm_wgmma.cu) leaves post-norm / post-RoPE K and V in the qkv
 // activation buffer next to q, and the shared prefix's K/V are kept per layer in a small
 // dense side buffer.  Dense rows are what TMA wants: every operand tile below is one or a
-// few cp.async.bulk.tensor boxes that land in shared memory already in the UMMA canonical
+// few cp.async.bulk.tensor boxes that land in shared memory already in the wgmma canonical
 // 128-byte-swizzled layout.  (The paged cache is still written by the epilogue — decode reads
 // it — and attn_prefill.cu remains the general paged-KV path for callers outside the engine.)
 //
 // Work item = (sequence, kv head, q tile).  A q tile packs QT = 128/G consecutive tokens x
-// the G query heads of the kv head into the 128 rows of one UMMA M tile (row = token*G +
-// head), so K/V are read once per GQA group and the causal frontier advances in QT-token
-// steps.  KV is consumed in blocks of up to 128 tokens: first the prefix blocks, then the
-// row's own blocks up to the tile's diagonal; the MMA N (and the PV K extent) is the valid
-// token count rounded up to 16, so short sequences do not pay for padding.
+// the G query heads of the kv head into 128 rows (row = token*G + head), so K/V are read once
+// per GQA group and the causal frontier advances in QT-token steps.  KV is consumed in blocks
+// of up to 128 tokens: first the prefix blocks, then the row's own blocks up to the tile's
+// diagonal.  Only the valid tokens (rounded up to 32-row TMA boxes) are loaded; the MMAs always
+// cover the whole 128-token block (a data-dependent wgmma count would make ptxas serialise
+// them), with P = 0 on the columns past the valid ones (selected, not multiplied, so garbage K
+// rows cannot leak into P).  0 * V stays 0 only where V is finite, so the CALLER must keep the
+// k/v columns of the qkv buffer and the prefix buffer finite in every row a 32-row box can reach
+// past a sequence's last token (the engine zeroes both buffers when it allocates them).  Rows
+// past the loaded ones hold an earlier block's V or the zeros the V ring starts with.
 //
-// Persistent CTA, 224 threads, one per SM, software-pipelined across blocks AND items:
-//   warps 4, 6  TMA producers Q tile (double-buffered) + K ring / V ring (2 stages each)
-//   warp 5      MMA issuer    S = Q K^T -> TMEM S[2];  O (+)= P V -> TMEM O[2]
-//   warps 0-3   softmax       thread == TMEM lane == tile row: tcgen05.ld S, running max with
-//                             lazy rescale (threshold 2^8), exp2, P -> shared memory (bf16,
-//                             K-major SW128), O rescale through tcgen05.ld/st when needed,
-//                             epilogue O / l -> global
-// Issue order of the MMA warp is S(g+1) before PV(g), so the tensor pipe computes the next
-// block's scores while the softmax warps work on the current one.
+// Persistent CTA, 384 threads, one per SM:
+//   warps 8-11  producer warpgroup (gives its registers to the consumers); warp 8 issues the
+//               TMA loads: the Q tile, then per block the K and V tiles (2-stage rings)
+//   warps 0-7   two consumer warpgroups, warpgroup c owns tile rows [64c, 64c+64):
+//               S = Q K^T  (wgmma, both operands from shared memory, S in registers);
+//               softmax in registers (a row lives in the four lanes of a quad): running max
+//               with lazy rescale (threshold 2^8), exp2, P packed to bf16 A fragments;
+//               O += P V   (wgmma, P from registers, V from shared memory MN-major);
+//               epilogue O / l -> global.
+// While one warpgroup runs its softmax the other one's MMAs keep the tensor cores busy.
 //
 // Results depend only on the sequence itself (block partition by absolute position, rescale
 // decisions per row), never on which other sequences share the batch.
@@ -34,19 +40,20 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace sb {
 
 namespace {
 
-constexpr int kTcThreads = 224;   // warps 0-3 softmax, 4 Q/K producer, 5 MMA issuer, 6 V producer
-constexpr int kBlk = 128;                    // KV tokens per block (TMEM S columns)
-constexpr int kHalfBytes = 128 * 128;        // [128 rows][64 bf16] = 16 KiB, one d-half / k-block
-constexpr int kTileBytes2 = 2 * kHalfBytes;  // 32 KiB: Q tile, K block, V block, P block
+constexpr int kTcThreads = 384;              // warps 0-7 consumers, warps 8-11 TMA producer
+constexpr int kBlk = 128;                    // KV tokens per block
+constexpr int kHalfBytes = 128 * 128;        // [128 rows][64 bf16] = 16 KiB, one d-half
+constexpr int kTileBytes2 = 2 * kHalfBytes;  // 32 KiB: Q tile, K block, V block
 constexpr int kBoxRows = 32;                 // K/V TMA box height
 constexpr int kBoxBytes = kBoxRows * 128;    // 4 KiB
 constexpr int kTcBarBytes = 256;
-constexpr int kTcSmem = 7 * kTileBytes2 + kTcBarBytes + 1024;  // Q[2] K[2] V[2] P + barriers + align
+constexpr int kTcSmem = 5 * kTileBytes2 + kTcBarBytes + 1024;  // Q K[2] V[2] + barriers + align
 constexpr float kRescaleThreshold = 8.0f;    // log2 units: P stays <= 2^8 before a forced rescale
 
 struct TcGeom {
@@ -91,27 +98,19 @@ SB_DEVICE void tc_block(const TcGeom& g, int b, bool& is_pre, int& j0, int& n16)
   n16 = (limit + 15) & ~15;
 }
 
-#ifdef SB200_ATTN_TRACE
-// Debug build only (tools/build_trace_lib.sh): CTA `g_tr_cta` stamps %clock at its pipeline
-// hand-offs, kTrCap stamps per role, for `tools/attn_bench.py --trace`.  The pointer lives in
-// the constant bank, so a stamp costs a compare, a CS2R and a store.  The product library is
-// compiled without the macro and carries none of it.
-constexpr int kTrCap = 1024;
-__constant__ long long* g_tr = nullptr;
-__constant__ int g_tr_cta = 0;
-#define TR(role, idx)                                                                   \
-  do {                                                                                  \
-    if (g_tr != nullptr && static_cast<int>(blockIdx.x) == g_tr_cta && (idx) < kTrCap)  \
-      g_tr[(role) * kTrCap + (idx)] = static_cast<long long>(clock());                 \
-  } while (0)
-#else
-#define TR(role, idx) do { } while (0)
-#endif
-
 SB_DEVICE float ex2_approx(float x) {   // MUFU.EX2: 2^x, flushes denormals (x <= -126 -> 0)
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
+}
+
+SB_DEVICE float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+SB_DEVICE float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
 template <int G>
@@ -123,69 +122,48 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
                        int n_items_total, const int32_t* __restrict__ seq_q_start,
                        const int32_t* __restrict__ seq_q_len, const int32_t* __restrict__ seq_past,
                        int hq, int hkv, int layer, float scale_log2) {
-  constexpr int QT = 128 / G;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  const uint32_t s_q = smem_u32(smem);                       // 2 x 32 KiB
-  const uint32_t s_k = s_q + 2 * kTileBytes2;                // 2 x 32 KiB
+  const uint32_t s_q = smem_u32(smem);                       // 32 KiB
+  const uint32_t s_k = s_q + kTileBytes2;                    // 2 x 32 KiB
   const uint32_t s_v = s_k + 2 * kTileBytes2;                // 2 x 32 KiB
-  const uint32_t s_p = s_v + 2 * kTileBytes2;                // 32 KiB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 7 * kTileBytes2);
-  // barrier indices
-  enum { Q_FULL = 0, Q_EMPTY = 2, K_FULL = 4, K_EMPTY = 6, V_FULL = 8, V_EMPTY = 10, S_FULL = 12,
-         S_EMPTY = 14, P_FULL = 16, P_EMPTY = 17, O_FULL = 18, O_EMPTY = 20, N_BARS = 22 };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + N_BARS);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 5 * kTileBytes2);
+  enum { Q_FULL = 0, Q_EMPTY = 1, K_FULL = 2, K_EMPTY = 4, V_FULL = 6, V_EMPTY = 8, N_BARS = 10 };
   auto bar = [&](int i) { return smem_u32(&bars[i]); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tm_q);
     tma_prefetch_desc(&tm_kv);
     tma_prefetch_desc(&tm_pre);
-  }
-  if (warp == 5 && lane == 0) {
     for (int i = 0; i < N_BARS; ++i) {
-      const bool from_softmax = (i >= S_EMPTY && i < S_EMPTY + 2) || i == P_FULL ||
-                                (i >= O_EMPTY && i < O_EMPTY + 2);
-      mbar_init(bar(i), from_softmax ? 4 : 1);  // softmax side: one arrival per warp
+      const bool from_consumers = i == Q_EMPTY || (i >= K_EMPTY && i < K_EMPTY + 2) ||
+                                  (i >= V_EMPTY && i < V_EMPTY + 2);
+      mbar_init(bar(i), from_consumers ? 8 : 1);  // consumer side: one arrival per warp
     }
     fence_mbar_init();
   }
-  if (warp == 0) {
-    tmem_alloc(smem_u32(tmem_slot), 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
+  for (int i = threadIdx.x; i < 2 * kTileBytes2 / 16; i += kTcThreads)
+    asm volatile("st.shared.v4.u32 [%0], {%1,%1,%1,%1};" ::"r"(s_v + 16 * i), "r"(0) : "memory");
+  fence_proxy_async_smem();   // the zeros are visible to the tensor cores' async proxy
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_s = tmem_base;        // S[sb] at columns sb*128
-  const uint32_t tmem_o = tmem_base + 256;  // O[ob] at columns 256 + ob*128
 
-  if (warp == 4 || warp == 6) {
-    // ===================== TMA producers =====================
-    // warp 4 streams Q tiles and K blocks, warp 6 the V blocks.  Two independent flows: a V
-    // stage frees up only when its P.V has retired (after the softmax), a K stage as soon as
-    // its S = Q.K^T has — one in-order producer would hold the next K block (and with it the
-    // next S) hostage behind the wait for the previous block's V stage.
-    const bool v_flow = warp == 6;
-    if (lane == 0) {
+  if (warp >= 8) {
+    // ===================== TMA producer =====================
+    // At most two blocks ahead of the consumers: block g's stage frees once block g-2 is done.
+    setmaxnreg_dec<40>();
+    if (warp == 8 && lane == 0) {
       uint32_t g = 0;  // global block counter of this CTA
       uint32_t n = 0;  // item counter of this CTA
       for (int item = blockIdx.x; item < n_items_total; item += gridDim.x, ++n) {
         const TcGeom ge = tc_geom<G>(item, hkv, items, seq_q_start, seq_q_len, seq_past);
-        if (!v_flow) {
-          const uint32_t qb = n & 1;
-          mbar_wait(bar(Q_EMPTY + qb), ((n >> 1) & 1) ^ 1);
-          mbar_arrive_expect_tx(bar(Q_FULL + qb), kTileBytes2);
-          const uint32_t qd = s_q + qb * kTileBytes2;
-          tma_load_3d(qd, &tm_q, bar(Q_FULL + qb), 0, ge.kvh * G, ge.q_start + ge.qt0);
-          tma_load_3d(qd + kHalfBytes, &tm_q, bar(Q_FULL + qb), 64, ge.kvh * G,
-                      ge.q_start + ge.qt0);
-        }
+        mbar_wait_long(bar(Q_EMPTY), (n & 1) ^ 1);
+        mbar_arrive_expect_tx(bar(Q_FULL), kTileBytes2);
+        tma_load_3d(s_q, &tm_q, bar(Q_FULL), 0, ge.kvh * G, ge.q_start + ge.qt0);
+        tma_load_3d(s_q + kHalfBytes, &tm_q, bar(Q_FULL), 64, ge.kvh * G, ge.q_start + ge.qt0);
         for (int b = 0; b < ge.n_blocks; ++b, ++g) {
           bool is_pre;
           int j0, n16;
@@ -193,305 +171,143 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
           const int n32 = (n16 + kBoxRows - 1) / kBoxRows;
           const uint32_t st = g & 1, ph = ((g >> 1) & 1) ^ 1;
           const int kcol = is_pre ? ge.kvh * kHeadDim : (hq + ge.kvh) * kHeadDim;
-          const int col = v_flow ? kcol + hkv * kHeadDim : kcol;
           const int row0 = is_pre ? j0 : ge.q_start + j0;
-          const uint32_t full = bar((v_flow ? V_FULL : K_FULL) + st);
-          const uint32_t base = (v_flow ? s_v : s_k) + st * kTileBytes2;
-          mbar_wait(bar((v_flow ? V_EMPTY : K_EMPTY) + st), ph);
-          TR(v_flow ? 1 : 0, 2 * g);
-          mbar_arrive_expect_tx(full, n32 * 2 * kBoxBytes);
-          for (int i = 0; i < n32; ++i) {
 #pragma unroll
-            for (int dh = 0; dh < 2; ++dh) {
-              const uint32_t dst = base + dh * kHalfBytes + i * kBoxBytes;
-              if (is_pre)
-                tma_load_3d(dst, &tm_pre, full, col + dh * 64, row0 + i * kBoxRows, layer);
-              else
-                tma_load_2d(dst, &tm_kv, full, col + dh * 64, row0 + i * kBoxRows);
-            }
-          }
-          TR(v_flow ? 1 : 0, 2 * g + 1);
-        }
-      }
-    }
-  } else if (warp == 5) {
-    // ===================== MMA issuer =====================
-    uint32_t g = 0, n = 0;
-    bool have_pending = false;
-    uint32_t p_g = 0, p_n16 = 0, p_ob = 0, p_opar = 0;
-    bool p_first = false, p_last = false;
-
-    auto do_pv = [&]() {
-      if (lane == 0) TR(3, 4 * p_g);
-      mbar_wait(bar(P_FULL), p_g & 1);
-      if (lane == 0) TR(3, 4 * p_g + 1);
-      mbar_wait(bar(V_FULL + (p_g & 1)), (p_g >> 1) & 1);
-      if (lane == 0) TR(3, 4 * p_g + 2);
-      if (p_first) mbar_wait(bar(O_EMPTY + p_ob), p_opar ^ 1);
-      if (lane == 0) TR(3, 4 * p_g + 3);
-      tc_fence_after();
-      if (lane == 0) {
-        const uint32_t st = p_g & 1;
-        const uint32_t d = tmem_o + p_ob * 128;
-        const uint32_t idesc = umma_idesc_bf16(128, 128) | kUmmaBMajorMN;
-        const int ksteps = static_cast<int>(p_n16) >> 4;
-        for (int kk = 0; kk < ksteps; ++kk) {
-          const uint64_t adesc = umma_desc_k_sw128(s_p + (kk >> 2) * kHalfBytes) + 2 * (kk & 3);
-          const uint64_t bdesc =
-              umma_desc_mn_sw128(s_v + st * kTileBytes2 + kk * 2048, kHalfBytes, 1024);
-          tc_mma_f16(d, adesc, bdesc, idesc, (p_first && kk == 0) ? 0u : 1u);
-        }
-        tc_commit(bar(V_EMPTY + st));
-        tc_commit(bar(P_EMPTY));
-        if (p_last) tc_commit(bar(O_FULL + p_ob));
-      }
-      __syncwarp();
-    };
-
-    for (int item = blockIdx.x; item < n_items_total; item += gridDim.x, ++n) {
-      const TcGeom ge = tc_geom<G>(item, hkv, items, seq_q_start, seq_q_len, seq_past);
-      const uint32_t qb = n & 1;
-      mbar_wait(bar(Q_FULL + qb), (n >> 1) & 1);
-      for (int b = 0; b < ge.n_blocks; ++b, ++g) {
-        bool is_pre;
-        int j0, n16;
-        tc_block<G>(ge, b, is_pre, j0, n16);
-        const uint32_t st = g & 1;
-        if (lane == 0) TR(2, 4 * g);
-        if (b == 0 && lane == 0) TR(2, 4 * g + 3);
-        mbar_wait(bar(K_FULL + st), (g >> 1) & 1);
-        if (lane == 0) TR(2, 4 * g + 1);
-        mbar_wait(bar(S_EMPTY + st), ((g >> 1) & 1) ^ 1);
-        if (lane == 0) TR(2, 4 * g + 2);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t idesc = umma_idesc_bf16(128, n16);
-          const uint32_t d = tmem_s + st * 128;
+          for (int v_flow = 0; v_flow < 2; ++v_flow) {
+            const int col = v_flow ? kcol + hkv * kHeadDim : kcol;
+            const uint32_t full = bar((v_flow ? V_FULL : K_FULL) + st);
+            const uint32_t base = (v_flow ? s_v : s_k) + st * kTileBytes2;
+            mbar_wait_long(bar((v_flow ? V_EMPTY : K_EMPTY) + st), ph);
+            mbar_arrive_expect_tx(full, n32 * 2 * kBoxBytes);
+            for (int i = 0; i < n32; ++i) {
 #pragma unroll
-          for (int dh = 0; dh < 2; ++dh) {
-            const uint64_t adesc = umma_desc_k_sw128(s_q + qb * kTileBytes2 + dh * kHalfBytes);
-            const uint64_t bdesc = umma_desc_k_sw128(s_k + st * kTileBytes2 + dh * kHalfBytes);
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              tc_mma_f16(d, adesc + 2 * k, bdesc + 2 * k, idesc, (dh | k) != 0 ? 1u : 0u);
-          }
-          tc_commit(bar(S_FULL + st));
-          tc_commit(bar(K_EMPTY + st));
-          if (b == ge.n_blocks - 1) tc_commit(bar(Q_EMPTY + qb));
-        }
-        __syncwarp();
-        if (have_pending) do_pv();
-        have_pending = true;
-        p_g = g;
-        p_n16 = static_cast<uint32_t>(n16);
-        p_ob = n & 1;
-        p_opar = (n >> 1) & 1;
-        p_first = b == 0;
-        p_last = b == ge.n_blocks - 1;
-      }
-    }
-    if (have_pending) do_pv();
-  } else {
-    // ===================== softmax / correction / epilogue (warps 0-3) =====================
-    const int r = warp * 32 + lane;       // tile row == TMEM lane
-    const int t_in = r / G;               // token within the q tile
-    const int h_in = r - t_in * G;        // query head within the GQA group
-    const uint32_t lane_sel = static_cast<uint32_t>(warp * 32) << 16;
-    const uint32_t p_row = s_p + r * 128;
-    const int sw = r & 7;
-    uint32_t g = 0, n = 0;
-    float m_used = 0.f, l_run = 0.f;
-    // The epilogue of an item is deferred until the first block of the NEXT item has been
-    // handed to the tensor core: the wait for the last P.V (O_FULL) then overlaps useful work
-    // instead of idling the softmax warps once per item (O is double-buffered).
-    bool ep_pending = false;
-    uint32_t ep_ob = 0, ep_par = 0;
-    float ep_inv = 0.f;
-    bool ep_row_ok = false;
-    __nv_bfloat16* ep_dst = nullptr;
-    auto flush_epilogue = [&]() {
-      if (!ep_pending) return;
-      ep_pending = false;
-      mbar_wait(bar(O_FULL + ep_ob), ep_par);
-      tc_fence_after();
-      const uint32_t o_addr = tmem_o + ep_ob * 128 + lane_sel;
-#pragma unroll 1
-      for (int half = 0; half < 2; ++half) {   // two 64-column halves: 64 live registers
-        uint32_t v[2][32];
-        tmem_ld_32x32(o_addr + half * 64, v[0]);
-        tmem_ld_32x32(o_addr + half * 64 + 32, v[1]);
-        tmem_ld_wait();
-        if (half == 1) {  // the accumulator has left TMEM: hand O[ob] back before the stores
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar(O_EMPTY + ep_ob));
-        }
-        if (ep_row_ok) {
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            uint32_t o[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-              o[i] = pack_bf16x2(__uint_as_float(v[c][2 * i]) * ep_inv,
-                                 __uint_as_float(v[c][2 * i + 1]) * ep_inv);
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              st_v4(ep_dst + half * 64 + c * 32 + 8 * i,
-                    make_uint4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]));
-          }
-        }
-      }
-    };
-    for (int item = blockIdx.x; item < n_items_total; item += gridDim.x, ++n) {
-      const TcGeom ge = tc_geom<G>(item, hkv, items, seq_q_start, seq_q_len, seq_past);
-      const int q_own = ge.qt0 + t_in;    // index of this row's token among the own tokens
-      const uint32_t ob = n & 1;
-      for (int b = 0; b < ge.n_blocks; ++b, ++g) {
-        bool is_pre;
-        int j0, n16;
-        tc_block<G>(ge, b, is_pre, j0, n16);
-        // columns c of this block are valid for this row iff c < vlim
-        const int vlim = min(is_pre ? ge.past - j0 : q_own - j0 + 1, n16);
-        const uint32_t sb = g & 1;
-        const int n_chunks = (n16 + 31) >> 5;
-        if (threadIdx.x == 0) TR(4, 8 * g);
-        mbar_wait(bar(S_FULL + sb), (g >> 1) & 1);
-        if (threadIdx.x == 0) TR(4, 8 * g + 1);
-        tc_fence_after();
-        const uint32_t s_addr = tmem_s + sb * 128 + lane_sel;
-        // ---- the whole score row into registers (one TMEM round trip), S[sb] released ----
-        uint32_t v[4][32];
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          if (c < n_chunks) tmem_ld_32x32(s_addr + c * 32, v[c]);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar(S_EMPTY + sb));
-        if (threadIdx.x == 0) TR(4, 8 * g + 2);
-        // One softmax warp per SM sub-partition: nothing hides ALU latency but ILP, and every
-        // instruction counts.  So (a) chunks that are valid for every row of the warp (all but
-        // the diagonal one: lane 0 holds the warp's smallest limit, limits grow with the lane)
-        // take a path without per-element predicates, (b) max and sum run on four independent
-        // accumulators, (c) exp2 is the bare MUFU (ex2.approx.ftz).
-        const int vmin = __shfl_sync(0xffffffffu, vlim, 0);
-        float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          if (c < n_chunks) {
-            if (c * 32 + 32 <= vmin) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(v[c][i]));
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (c * 32 + i < vlim) mx4[i & 3] = fmaxf(mx4[i & 3], __uint_as_float(v[c][i]));
-            }
-          }
-        float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-        mx *= scale_log2;  // scale > 0: max commutes with the scaling
-        if (threadIdx.x == 0) TR(5, 4 * g);
-        // ---- running max with lazy rescale ----
-        float alpha = 1.f;
-        bool need = false;
-        if (b == 0) {
-          m_used = (mx == -INFINITY) ? 0.f : mx;
-          l_run = 0.f;
-        } else if (mx > m_used + kRescaleThreshold) {
-          alpha = ex2_approx(m_used - mx);
-          m_used = mx;
-          l_run *= alpha;
-          need = true;
-        }
-        // ---- P = exp2(s*scale - m) -> bf16 (registers) ----
-        float ps4[4] = {0.f, 0.f, 0.f, 0.f};
-        const float neg_m = -m_used;
-        if (threadIdx.x == 0) TR(5, 4 * g + 1);
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          if (c < n_chunks) {
-            if (c * 32 + 32 <= vmin) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {   // packed pairs overwrite the scores in place
-                const float p0 = ex2_approx(fmaf(__uint_as_float(v[c][2 * i]), scale_log2, neg_m));
-                const float p1 =
-                    ex2_approx(fmaf(__uint_as_float(v[c][2 * i + 1]), scale_log2, neg_m));
-                ps4[i & 3] += p0 + p1;
-                v[c][i] = pack_bf16x2(p0, p1);
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const int c0 = c * 32 + 2 * i;
-                float p0 = ex2_approx(fmaf(__uint_as_float(v[c][2 * i]), scale_log2, neg_m));
-                float p1 = ex2_approx(fmaf(__uint_as_float(v[c][2 * i + 1]), scale_log2, neg_m));
-                p0 = c0 < vlim ? p0 : 0.f;
-                p1 = c0 + 1 < vlim ? p1 : 0.f;
-                ps4[i & 3] += p0 + p1;
-                v[c][i] = pack_bf16x2(p0, p1);
+              for (int dh = 0; dh < 2; ++dh) {
+                const uint32_t dst = base + dh * kHalfBytes + i * kBoxBytes;
+                if (is_pre)
+                  tma_load_3d(dst, &tm_pre, full, col + dh * 64, row0 + i * kBoxRows, layer);
+                else
+                  tma_load_2d(dst, &tm_kv, full, col + dh * 64, row0 + i * kBoxRows);
               }
             }
           }
-        const float psum = (ps4[0] + ps4[1]) + (ps4[2] + ps4[3]);
-        l_run += psum;
-        // the previous block's PV must have retired before O is rescaled or P is overwritten
-        if (threadIdx.x == 0) TR(4, 8 * g + 3);
-        mbar_wait(bar(P_EMPTY), (g & 1) ^ 1);
-        if (threadIdx.x == 0) TR(4, 8 * g + 4);
-        if (__any_sync(0xffffffffu, need)) {
-          tc_fence_after();
-          const uint32_t o_addr = tmem_o + ob * 128 + lane_sel;
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            uint32_t o[32];
-            tmem_ld_32x32(o_addr + c * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_32x32(o_addr + c * 32, o);
-          }
-          tmem_st_wait();
-          tc_fence_before();
-        }
-        // ---- P -> shared memory (K-major, SW128): 32 columns = four 16-byte chunks ----
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          if (c < n_chunks) {
-            const uint32_t base = p_row + (c >> 1) * kHalfBytes;
-#pragma unroll
-            for (int q4 = 0; q4 < 4; ++q4) {
-              const int cc = (c & 1) * 4 + q4;
-              asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(base + ((cc ^ sw) << 4)),
-                           "r"(v[c][4 * q4]), "r"(v[c][4 * q4 + 1]), "r"(v[c][4 * q4 + 2]),
-                           "r"(v[c][4 * q4 + 3])
-                           : "memory");
-            }
-          }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar(P_FULL));
-        if (threadIdx.x == 0) TR(4, 8 * g + 5);
-        flush_epilogue();
-        if (threadIdx.x == 0) TR(4, 8 * g + 6);   // the previous item's, if any: the tensor core is busy with this block
-        if (b == ge.n_blocks - 1) {
-          ep_pending = true;
-          ep_ob = ob;
-          ep_par = (n >> 1) & 1;
-          ep_inv = 1.0f / l_run;
-          ep_row_ok = q_own < ge.q_len;
-          ep_dst = out + static_cast<size_t>(ge.q_start + q_own) * (hq * kHeadDim) +
-                   (ge.kvh * G + h_in) * kHeadDim;
         }
       }
     }
-    flush_epilogue();
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // ===================== consumers (warps 0-7) =====================
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2;
+  const int q4 = lane & 3;
+  const uint32_t s_qw = s_q + wg * 64 * 128;       // this warpgroup's 64 Q rows
+  int t_in[2], h_in[2];                            // token / query head of the thread's 2 rows
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+    t_in[h] = r / G;
+    h_in[h] = r - t_in[h] * G;
+  }
+  uint32_t g = 0, n = 0;
+  for (int item = blockIdx.x; item < n_items_total; item += gridDim.x, ++n) {
+    const TcGeom ge = tc_geom<G>(item, hkv, items, seq_q_start, seq_q_len, seq_past);
+    float o[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    float m_used[2] = {0.f, 0.f}, l_run[2] = {0.f, 0.f};   // l_run: this thread's partial sums
+    mbar_wait(bar(Q_FULL), n & 1);
+    for (int b = 0; b < ge.n_blocks; ++b, ++g) {
+      bool is_pre;
+      int j0, n16;
+      tc_block<G>(ge, b, is_pre, j0, n16);
+      const uint32_t st = g & 1, par = (g >> 1) & 1;
+      // ---- S = Q K^T (64 x 128 per warpgroup) ----
+      float s[64];
+      mbar_wait(bar(K_FULL + st), par);
+      wgmma_fence();
+#pragma unroll
+      for (int dh = 0; dh < 2; ++dh)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n128k16_ss(s, gmma_desc_k_sw128(s_qw + dh * kHalfBytes + 32 * k),
+                              gmma_desc_k_sw128(s_k + st * kTileBytes2 + dh * kHalfBytes + 32 * k),
+                              (dh | k) != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(bar(K_EMPTY + st));
+        if (b == ge.n_blocks - 1) mbar_arrive(bar(Q_EMPTY));
+      }
+      // ---- softmax: s[4j + 2h + e] is row h, column 8j + 2 q4 + e of the block ----
+      uint32_t pa[32];   // P as bf16x2: the A fragments of the eight K=16 steps of P.V
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        // columns c of this block are valid for this row iff c < vlim
+        const int vlim = min(is_pre ? ge.past - j0 : ge.qt0 + t_in[h] - j0 + 1, n16);
+        float mx = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (8 * j + 2 * q4 + e < vlim) mx = fmaxf(mx, s[4 * j + 2 * h + e]);
+        mx = quad_max(mx) * scale_log2;   // scale > 0: max commutes with the scaling
+        if (b == 0) {
+          m_used[h] = (mx == -INFINITY) ? 0.f : mx;
+        } else if (mx > m_used[h] + kRescaleThreshold) {
+          const float alpha = ex2_approx(m_used[h] - mx);
+          m_used[h] = mx;
+          l_run[h] *= alpha;
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            o[4 * j + 2 * h] *= alpha;
+            o[4 * j + 2 * h + 1] *= alpha;
+          }
+        }
+        const float neg_m = -m_used[h];
+        float ps = 0.f;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int c0 = 8 * j + 2 * q4;
+          float p0 = ex2_approx(fmaf(s[4 * j + 2 * h], scale_log2, neg_m));
+          float p1 = ex2_approx(fmaf(s[4 * j + 2 * h + 1], scale_log2, neg_m));
+          p0 = c0 < vlim ? p0 : 0.f;
+          p1 = c0 + 1 < vlim ? p1 : 0.f;
+          ps += p0 + p1;
+          // K step kk = j / 2: a0/a1 = rows 0/8 at k 2q4, a2/a3 = rows 0/8 at k 8 + 2q4
+          pa[4 * (j >> 1) + 2 * (j & 1) + h] = pack_bf16x2(p0, p1);
+        }
+        l_run[h] += ps;
+      }
+      // ---- O += P V ----
+      mbar_wait(bar(V_FULL + st), par);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+        wgmma_m64n128k16_rs_tb(
+            o, a, gmma_desc_sw128(s_v + st * kTileBytes2 + kk * 2048, kHalfBytes, 1024));
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar(V_EMPTY + st));
+    }
+    // ---- epilogue: O / l -> bf16 -> global ----
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float inv = 1.0f / quad_sum(l_run[h]);
+      const int q_own = ge.qt0 + t_in[h];
+      if (q_own >= ge.q_len) continue;
+      __nv_bfloat16* dst = out + static_cast<size_t>(ge.q_start + q_own) * (hq * kHeadDim) +
+                           (ge.kvh * G + h_in[h]) * kHeadDim + 2 * q4;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        *reinterpret_cast<uint32_t*>(dst + 8 * j) =
+            pack_bf16x2(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
+    }
   }
 }
 
@@ -566,7 +382,7 @@ int tc_num_sms() {
   int dev = 0, n = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  return n > 0 ? n : 148;
+  return n > 0 ? n : 1;
 }
 
 template <int G>
@@ -618,11 +434,3 @@ int attn_prefill_dense(const void* qkv, int t_rows, void* out, const void* prefi
 }
 
 }  // namespace sb
-
-#ifdef SB200_ATTN_TRACE
-extern "C" int sb200_attn_trace(long long* dev_buf, int cta) {
-  if (cudaMemcpyToSymbol(sb::g_tr, &dev_buf, sizeof(dev_buf)) != cudaSuccess) return -1;
-  if (cudaMemcpyToSymbol(sb::g_tr_cta, &cta, sizeof(cta)) != cudaSuccess) return -1;
-  return 0;
-}
-#endif

@@ -1,8 +1,8 @@
-// sutro_b200 — shared device helpers (sm_100a only).
+// sutro_b200 — shared device helpers (sm_90a).
 //
-// Thin inline-PTX wrappers for the Blackwell async machinery used by the
-// kernels in this directory: mbarrier, bulk/tensor TMA, tcgen05 (TMEM alloc,
-// MMA, commit, ld), plus the usual warp reductions and bf16 packing.
+// Thin inline-PTX wrappers for the Hopper async machinery used by the kernels in
+// this directory: mbarrier and bulk/tensor TMA (the wgmma wrappers are in
+// wgmma.cuh), plus the usual warp reductions and bf16 packing.
 #pragma once
 
 #include <cuda.h>
@@ -115,6 +115,17 @@ SB_DEVICE void st_v4(void* p, const uint4& v) {
                : "memory");
 }
 
+// Warpgroup register budget (sm_90a): the TMA producer warpgroup hands its registers to the
+// MMA warpgroups.  Executed by every thread of the warpgroup; counts are multiples of 8.
+template <int N>
+SB_DEVICE void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+SB_DEVICE void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // ---------------------------------------------------------------------------
 // mbarrier
 // ---------------------------------------------------------------------------
@@ -202,244 +213,7 @@ SB_DEVICE void bulk_load_1d(uint32_t smem_dst, const void* gsrc, uint32_t bytes,
 }
 
 // ---------------------------------------------------------------------------
-// tcgen05 / TMEM
-// ---------------------------------------------------------------------------
-SB_DEVICE void tmem_alloc(uint32_t smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_result),
-               "r"(ncols)
-               : "memory");
-}
-SB_DEVICE void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-SB_DEVICE void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-SB_DEVICE void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-SB_DEVICE void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; single elected thread issues.
-SB_DEVICE void tc_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued MMAs have retired.
-SB_DEVICE void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   bar)
-               : "memory");
-}
-SB_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns: thread i gets row (lane base + i).
-SB_DEVICE void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns, registers -> TMEM (thread i writes row lane base + i).
-SB_DEVICE void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-      "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),
-      "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]),
-      "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]),
-      "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-SB_DEVICE void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---- cta_group::2 (CTA pair) variants ------------------------------------
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // shared::cluster address of the even CTA
-
-SB_DEVICE uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-SB_DEVICE void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// 2-CTA TMA load: data lands in this CTA's smem, bytes are counted on the leader's barrier.
-SB_DEVICE void tma_load_2d_cta2(uint32_t smem_dst, const CUtensorMap* m, uint32_t leader_bar,
-                                int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_dst),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(leader_bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-SB_DEVICE void tmem_alloc_cta2(uint32_t smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_result),
-               "r"(ncols)
-               : "memory");
-}
-SB_DEVICE void tmem_relinquish_cta2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-SB_DEVICE void tmem_dealloc_cta2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-SB_DEVICE void tc_mma_f16_cta2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                               uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// ---- one K block per asm statement -------------------------------------------------------
-// The thread that issues tcgen05.mma is alone on its job: per 64-element K block the tensor
-// pipe needs 512 cycles (128x256x64 per SM) and the thread must get four MMAs and a commit out
-// in less.  Written as five separate asm statements with 64-bit descriptor operands that costs
-// ~124 SASS instructions (ptxas moves every operand into uniform registers with an ELECT +
-// R2UR.BROADCAST round trip per instruction and does the 64-bit descriptor arithmetic in
-// register pairs) — at the IPC one warp reaches that IS the 512 cycles, and ncu showed the issuing
-// thread busy 85 % of the time with the tensor pipe 84 % active.  Here the descriptor's high
-// word is an immediate (SBO = 1024 B, version 1, SWIZZLE_128B: constant for every K-major
-// SW128 tile), only the low words (start address | LBO) travel, and the +32-byte K steps are
-// 32-bit adds.
-constexpr uint32_t kDescHiKSw128 = (1024u >> 4) | (1u << 14) | (2u << 29);   // = 0x40004040
-SB_DEVICE uint32_t umma_desc_lo_k_sw128(uint32_t smem_addr) {
-  return ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16);
-}
-#define SB_KBLOCK4_BODY(GROUP)                                                               \
-  ".reg .pred p;\n"                                                                          \
-  ".reg .b64 da, db;\n"                                                                      \
-  ".reg .b32 al, bl;\n"                                                                      \
-  "setp.ne.b32 p, %4, 0;\n"                                                                  \
-  "mov.b64 da, {%1, %5};\n"                                                                  \
-  "mov.b64 db, {%2, %5};\n"                                                                  \
-  "tcgen05.mma.cta_group::" GROUP ".kind::f16 [%0], da, db, %3, p;\n"                        \
-  "setp.ne.b32 p, 1, 0;\n"                                                                   \
-  "add.u32 al, %1, 2;\n"                                                                     \
-  "add.u32 bl, %2, 2;\n"                                                                     \
-  "mov.b64 da, {al, %5};\n"                                                                  \
-  "mov.b64 db, {bl, %5};\n"                                                                  \
-  "tcgen05.mma.cta_group::" GROUP ".kind::f16 [%0], da, db, %3, p;\n"                        \
-  "add.u32 al, %1, 4;\n"                                                                     \
-  "add.u32 bl, %2, 4;\n"                                                                     \
-  "mov.b64 da, {al, %5};\n"                                                                  \
-  "mov.b64 db, {bl, %5};\n"                                                                  \
-  "tcgen05.mma.cta_group::" GROUP ".kind::f16 [%0], da, db, %3, p;\n"                        \
-  "add.u32 al, %1, 6;\n"                                                                     \
-  "add.u32 bl, %2, 6;\n"                                                                     \
-  "mov.b64 da, {al, %5};\n"                                                                  \
-  "mov.b64 db, {bl, %5};\n"                                                                  \
-  "tcgen05.mma.cta_group::" GROUP ".kind::f16 [%0], da, db, %3, p;\n"
-// Four K=16 steps of one SW128 K block (A, B both K-major) + the commit that frees the stage.
-// Called by the ONE issuing thread.
-SB_DEVICE void tc_mma_kblock4_cta2(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t idesc,
-                                   uint32_t accumulate_first, uint32_t empty_bar, uint16_t mask) {
-  asm volatile(
-      "{\n" SB_KBLOCK4_BODY("2")
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%6], %7;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate_first), "n"(kDescHiKSw128), "r"(empty_bar),
-      "h"(mask)
-      : "memory");
-}
-SB_DEVICE void tc_mma_kblock4(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t idesc,
-                              uint32_t accumulate_first, uint32_t empty_bar) {
-  asm volatile(
-      "{\n" SB_KBLOCK4_BODY("1")
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%6];\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate_first), "n"(kDescHiKSw128), "r"(empty_bar)
-      : "memory");
-}
-// the same four steps without a commit: the first half of a two-span (K = 128) stage
-SB_DEVICE void tc_mma_kblock4_cta2_nocommit(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo,
-                                            uint32_t idesc, uint32_t accumulate_first) {
-  asm volatile(
-      "{\n" SB_KBLOCK4_BODY("2")
-      "}\n" ::"r"(tmem_d),
-      "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate_first), "n"(kDescHiKSw128)
-      : "memory");
-}
-#undef SB_KBLOCK4_BODY
-// commit: arrive on the barrier at this offset in every CTA of `mask`
-SB_DEVICE void tc_commit_cta2_mc(uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;" ::"r"(bar),
-      "h"(mask)
-      : "memory");
-}
-SB_DEVICE void mbar_arrive_cluster(uint32_t cluster_bar_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar_addr) : "memory");
-}
-
-// K-major, 128-byte-swizzled operand tile: rows at 128 B pitch, 8-row groups
-// every 1024 B (SBO), descriptor version 1 (Blackwell), layout SWIZZLE_128B.
-// (cf. cute::UMMA::SmemDescriptor bit layout.)
-SB_DEVICE uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);  // start address  [0,14)
-  d |= static_cast<uint64_t>(1) << 16;                      // LBO (unused)   [16,30)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;              // SBO = 1024 B   [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                      // version = 1
-  d |= static_cast<uint64_t>(2) << 61;                      // SWIZZLE_128B
-  return d;
-}
-
-// MN-major, 128-byte-swizzled operand tile (cf. cute::UMMA::make_umma_desc<Major::MN>): the
-// MN dimension is contiguous in 64-element (128 B) spans; 8 consecutive K rows (128 B pitch)
-// form one 1024-byte swizzle atom.  SBO = byte distance between 8-row K groups, LBO = byte
-// distance between 64-element MN spans.
-SB_DEVICE uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);        // start address  [0,14)
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;   // LBO            [16,30)
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;   // SBO            [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                            // version = 1
-  d |= static_cast<uint64_t>(2) << 61;                            // SWIZZLE_128B
-  return d;
-}
-constexpr uint32_t kUmmaBMajorMN = 1u << 16;  // instruction-descriptor bit: B operand MN-major
-
-// kind::f16 instruction descriptor: bf16 x bf16 -> fp32, both operands K-major.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int m, int n) {
-  return (1u << 4)                               // C format F32
-         | (1u << 7)                             // A format BF16
-         | (1u << 10)                            // B format BF16
-         | (static_cast<uint32_t>(n >> 3) << 17) // N / 8
-         | (static_cast<uint32_t>(m >> 4) << 24);  // M / 16
-}
-
-// ---------------------------------------------------------------------------
-// legacy-path tensor core helpers used by the attention kernels
+// mma.sync tensor core helpers used by the paged attention kernels
 // ---------------------------------------------------------------------------
 SB_DEVICE void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
   asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"

@@ -220,7 +220,7 @@ struct Engine {
   double gemm_flops = 0, attn_decode_bytes = 0;
   int device = 0;
   bool fuse_qkv = true;  // SB200_FUSE_QKV=0 keeps the separate rope_kv_write kernel (A/B tests)
-  // tcgen05 prefill attention over dense K/V (attn_prefill_tc.cu); SB200_PREFILL_TC=0 falls
+  // wgmma prefill attention over dense K/V (attn_prefill_tc.cu); SB200_PREFILL_TC=0 falls
   // back to the paged mma.sync kernel (A/B tests)
   bool prefill_tc = true;
   bf16* prefix_kv = nullptr;  // [n_layers][prefix_rows][2*hkv*128]: dense K|V of the shared prefix

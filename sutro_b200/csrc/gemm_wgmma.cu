@@ -1,0 +1,609 @@
+// sutro_b200 — K1: bf16 GEMM  D[M,N] = A[M,K] · W[N,K]^T  on Hopper wgmma tensor cores.
+//
+// Every projection of the transformer (QKV, O, gate/up, down, lm_head) has this
+// shape: activations row-major [tokens, K], weights row-major [N, K] — both
+// K-major, which is the native operand layout of wgmma with 128-byte swizzled
+// shared-memory tiles.
+//
+// Kernel anatomy (persistent, warp-specialised, one CTA per SM, 384 threads):
+//   warps 0-7  two consumer warpgroups: warpgroup c owns rows [64c, 64c+64) of the 128-row
+//              tile and issues wgmma.m64nBLOCK_Nk16 (four per 64-element K block) straight
+//              from the shared-memory ring, accumulating in registers; one K block stays in
+//              flight while the next is issued.  The fused epilogue runs from the registers.
+//   warps 8-11 producer warpgroup (gives its registers to the consumers); warp 8 issues the
+//              cp.async.bulk.tensor 2-D loads of A (128x64) and W (BLOCK_N x 64) tiles into a
+//              kStages-deep ring and runs ahead into the next tile while the consumers are in
+//              their epilogue.
+//
+// Fused epilogues (rounding points mirror the bf16 oracle, oracle/model_ref.py):
+//   STORE_BF16     D = bf16(acc)
+//   RESIDUAL_BF16  D = bf16(bf16(acc) + R)           (O-proj / down-proj + residual)
+//   SWIGLU_BF16    D[:, j] = bf16(silu(bf16(acc[2j])) * bf16(acc[2j+1]))
+//                  (gate/up weights interleaved row-wise; output has N/2 columns)
+//   STORE_F32      D = acc                             (lm_head logits)
+//   QKV_ROPE       q/k RMSNorm + RoPE, K/V into the paged cache (see qkv_head_epilogue)
+#include <algorithm>
+#include <cstdlib>
+#include <mutex>
+#include <unordered_map>
+
+#include "common.cuh"
+#include "kernels.h"
+#include "wgmma.cuh"
+
+namespace sb {
+
+namespace {
+
+constexpr int kBlockM = 128;
+constexpr int kBlockK = 64;   // 64 bf16 = 128 B = one swizzle span
+constexpr int kConsumerWarps = 8;
+constexpr int kProducerWarp = kConsumerWarps;
+constexpr int kGemmThreads = 32 * (kConsumerWarps + 4);
+
+template <int BLOCK_N>
+struct GemmCfg {
+  static constexpr int kABytes = kBlockM * kBlockK * 2;
+  static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
+  static constexpr int kStageBytes = kABytes + kBBytes;
+  // ~192 KiB of ring for every tile width (the limit is 227 KiB per block)
+  static constexpr int kStages = (BLOCK_N == 256) ? 4 : (BLOCK_N == 128 ? 6 : 8);
+  static constexpr int kBarBytes = 256;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kBarBytes + 1024;  // +align slack
+};
+
+template <int BN>
+SB_DEVICE void wgmma_ss(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc) {
+  if constexpr (BN == 64) wgmma_m64n64k16_ss(d, adesc, bdesc, 1);
+  else if constexpr (BN == 128) wgmma_m64n128k16_ss(d, adesc, bdesc, 1);
+  else wgmma_m64n256k16_ss(d, adesc, bdesc, 1);
+}
+
+// Tile rasterisation: consecutive tile ids sweep all N tiles of a group of GM row-tiles
+// before moving on, so the CTAs running concurrently share a [GM*128, K] slab of A and a
+// slab of W that both stay in L2 (M-fastest order would re-read A from HBM once per N tile).
+SB_DEVICE void tile_to_mn(int GM, int tile, int num_m, int num_n, int& m_blk, int& n_blk) {
+  const int group_tiles = GM * num_n;
+  const int g = tile / group_tiles;
+  const int first_m = g * GM;
+  const int gm = min(GM, num_m - first_m);
+  const int within = tile - g * group_tiles;
+  m_blk = first_m + within % gm;
+  n_blk = within / gm;
+}
+
+// This thread's accumulators (rows row0 and row0 + 8, columns col0 + 8j + {0, 1}) -> fused
+// epilogue -> global.  col0 already includes the lane's 2 * (lane % 4).
+template <int BLOCK_N, int EPI>
+SB_DEVICE void epilogue_store(const float (&acc)[BLOCK_N / 2], void* __restrict__ d_out,
+                              const __nv_bfloat16* __restrict__ resid, int row0, int col0, int M,
+                              int N, int ldd) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 8 * h;
+      const bool ok = col < N && row < M;
+      const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      const size_t off = static_cast<size_t>(row) * ldd + col;
+      if constexpr (EPI == EPI_SWIGLU_BF16) {
+        const float g = bf16_round(v0);
+        const float u = bf16_round(v1);
+        const float s = bf16_round(g / (1.0f + __expf(-g)));
+        // output column col/2: the even lane of a pair stores its own and its neighbour's
+        const uint32_t mine = __bfloat16_as_ushort(__float2bfloat16_rn(s * u));
+        const uint32_t other = __shfl_xor_sync(0xffffffffu, mine, 1);
+        if (ok && (lane & 1) == 0)
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(d_out) +
+                                       static_cast<size_t>(row) * ldd + (col >> 1)) =
+              mine | (other << 16);
+      } else if (ok) {
+        if constexpr (EPI == EPI_STORE_F32) {
+          *reinterpret_cast<float2*>(reinterpret_cast<float*>(d_out) + off) = make_float2(v0, v1);
+        } else if constexpr (EPI == EPI_RESIDUAL_BF16) {
+          const float2 r = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(resid + off));
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(d_out) + off) =
+              pack_bf16x2(bf16_round(v0) + r.x, bf16_round(v1) + r.y);
+        } else {
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(d_out) + off) =
+              pack_bf16x2(v0, v1);
+        }
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------
+// EPI_QKV_ROPE: per 128-column head, each row gets exactly what rope_kv_kernel (norm_rope.cu)
+// does to the stored bf16 tensor — bf16 rounding of the projection, optional per-head RMSNorm,
+// rotate-half RoPE with bf16 op-by-op rounding — then q heads go to the qkv buffer and k/v
+// heads straight into the swizzled KV page (and, unswizzled, into their columns of the qkv
+// buffer for the dense prefill attention).  A row's head is spread over the four lanes of a
+// quad (32 dims each); dim d and its RoPE partner d + 64 sit in the same thread, so only the
+// sum of squares needs two shuffles.
+// ---------------------------------------------------------------------------
+struct QkvRowMeta {
+  int pos, r;
+  size_t page;
+};
+
+SB_DEVICE void qkv_row_meta(const QkvEpiArgs& ea, int row, bool row_ok, QkvRowMeta& rm) {
+  rm.pos = 0, rm.r = 0, rm.page = 0;
+  if (row_ok) {
+    rm.pos = ea.tok_pos[row];
+    const int slot = ea.tok_slot[row];
+    rm.page = static_cast<size_t>(
+        ea.page_table[static_cast<size_t>(slot) * ea.max_pages + rm.pos / kPageTokens]);
+    rm.r = rm.pos % kPageTokens;
+  }
+}
+
+template <int R>
+SB_DEVICE void qkv_head_epilogue(const float (&acc)[R], int hh, const QkvEpiArgs& ea,
+                                 const QkvRowMeta (&rm)[2], int row0, int M, int head, bool head_ok,
+                                 __nv_bfloat16* __restrict__ qkv_out, int ldd) {
+  const int q = threadIdx.x & 3;
+  const bool is_q = head < ea.hq;
+  const bool is_k = !is_q && head < ea.hq + ea.hkv;
+  const __nv_bfloat16* nw =
+      static_cast<const __nv_bfloat16*>(is_q ? ea.q_norm_w : (is_k ? ea.k_norm_w : nullptr));
+  // Packed bf16x2 arithmetic: a product of two bf16 values is exact in fp32, so HMUL2.BF16
+  // (one rounding) equals "fp32 multiply, round to bf16" — the rounding points of the unfused
+  // kernel (norm_rope.cu) and of the oracle; sums are HADD2.BF16 (exact sum, one rounding).
+  // explicit .rn forms: ptxas must not contract mul + add/sub into one fused (singly rounded) FMA
+  auto mul2 = [](uint32_t a, uint32_t b) {
+    uint32_t d;
+    asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
+    return d;
+  };
+  auto add2 = [](uint32_t a, uint32_t b) {
+    uint32_t d;
+    asm("add.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
+    return d;
+  };
+  auto sub2 = [](uint32_t a, uint32_t b) {
+    uint32_t d;
+    asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
+    return d;
+  };
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + 8 * h;
+    // 32 fp32 accumulators -> 16 packed bf16x2 (the rounding of the linear output):
+    // u[jj] holds dims 8jj + 2q, +1 of the head
+    uint32_t u[16];
+    float ss = 0.f;
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      const int i = 4 * (16 * hh + jj) + 2 * h;
+      u[jj] = pack_bf16x2(acc[i], acc[i + 1]);
+      const float2 f = unpack_bf16x2(u[jj]);
+      ss += f.x * f.x + f.y * f.y;
+    }
+    ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+    ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+    if (!head_ok || row >= M) continue;
+    const float rstd = nw != nullptr ? rsqrtf(ss / static_cast<float>(kHeadDim) + ea.eps) : 1.f;
+    __nv_bfloat16* dst_lo;
+    __nv_bfloat16* dense = qkv_out + static_cast<size_t>(row) * ldd + head * kHeadDim;
+    int swz = 0;
+    if (is_q) {
+      dst_lo = dense;
+    } else {
+      const int kvh = is_k ? (head - ea.hq) : (head - ea.hq - ea.hkv);
+      dst_lo = static_cast<__nv_bfloat16*>(ea.kv_layer) +
+               (rm[h].page * ea.hkv + kvh) * (2 * kTileElems) + (is_k ? 0 : kTileElems) +
+               rm[h].r * kHeadDim;
+      swz = rm[h].r & 7;
+    }
+    const __nv_bfloat16* cosr =
+        static_cast<const __nv_bfloat16*>(ea.cos_tab) + static_cast<size_t>(rm[h].pos) * 64;
+    const __nv_bfloat16* sinr =
+        static_cast<const __nv_bfloat16*>(ea.sin_tab) + static_cast<size_t>(rm[h].pos) * 64;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {   // dims d, d+1 of the low half and their +64 partners
+      const int d = 8 * jj + 2 * q;
+      uint32_t lo = u[jj], hi = u[jj + 8];
+      if (nw != nullptr) {   // w * bf16(x * rstd): rstd is fp32, so that product is fp32
+        const float2 a = unpack_bf16x2(lo), b = unpack_bf16x2(hi);
+        lo = mul2(*reinterpret_cast<const uint32_t*>(nw + d), pack_bf16x2(a.x * rstd, a.y * rstd));
+        hi = mul2(*reinterpret_cast<const uint32_t*>(nw + 64 + d),
+                  pack_bf16x2(b.x * rstd, b.y * rstd));
+      }
+      if (is_q || is_k) {
+        // out[i] = x[i]*cos - x[i+64]*sin ; out[i+64] = x[i+64]*cos + x[i]*sin (bf16 op by op)
+        const uint32_t c = *reinterpret_cast<const uint32_t*>(cosr + d);
+        const uint32_t s = *reinterpret_cast<const uint32_t*>(sinr + d);
+        const uint32_t x = lo, y = hi;
+        lo = sub2(mul2(x, c), mul2(y, s));
+        hi = add2(mul2(y, c), mul2(x, s));
+      }
+      *reinterpret_cast<uint32_t*>(dst_lo + ((jj ^ swz) << 3) + 2 * q) = lo;
+      *reinterpret_cast<uint32_t*>(dst_lo + (((jj + 8) ^ swz) << 3) + 2 * q) = hi;
+      if (!is_q && ea.write_dense) {
+        // dense copy next to q: the dense prefill attention reads the new tokens' K/V from the
+        // qkv buffer through TMA (attn_prefill_tc.cu); decode reads the paged copy above
+        *reinterpret_cast<uint32_t*>(dense + d) = lo;
+        *reinterpret_cast<uint32_t*>(dense + 64 + d) = hi;
+      }
+    }
+  }
+}
+
+template <int BLOCK_N, int EPI>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
+                    const __grid_constant__ CUtensorMap tm_b, void* __restrict__ d_out,
+                    const __nv_bfloat16* __restrict__ resid, int M, int N, int K, int ldd,
+                    int ea_gm, const QkvEpiArgs ea) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  extern __shared__ uint8_t smem_raw[];
+  // SWIZZLE_128B tiles need 1024-byte alignment.
+  uint8_t* smem = reinterpret_cast<uint8_t*>(
+      (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* full_bar = bars;
+  uint64_t* empty_bar = bars + Cfg::kStages;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (warp == kProducerWarp && lane == 0) {
+    tma_prefetch_desc(&tm_a);
+    tma_prefetch_desc(&tm_b);
+    for (int s = 0; s < Cfg::kStages; ++s) {
+      mbar_init(smem_u32(&full_bar[s]), 1);
+      mbar_init(smem_u32(&empty_bar[s]), kConsumerWarps);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const int num_m = (M + kBlockM - 1) / kBlockM;
+  const int num_n = (N + BLOCK_N - 1) / BLOCK_N;
+  const int num_tiles = num_m * num_n;
+  const int num_k = K / kBlockK;
+
+  if (warp >= kProducerWarp) {
+    // ===== TMA producer =====
+    setmaxnreg_dec<40>();
+    if (warp == kProducerWarp && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int m_blk, n_blk;
+        tile_to_mn(ea_gm, tile, num_m, num_n, m_blk, n_blk);
+        for (int kb = 0; kb < num_k; ++kb) {
+          mbar_wait_long(smem_u32(&empty_bar[stage]), phase ^ 1);
+          const uint32_t fb = smem_u32(&full_bar[stage]);
+          const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
+          mbar_arrive_expect_tx(fb, Cfg::kStageBytes);
+          tma_load_2d(sa, &tm_a, fb, kb * kBlockK, m_blk * kBlockM);
+          tma_load_2d(sa + Cfg::kABytes, &tm_b, fb, kb * kBlockK, n_blk * BLOCK_N);
+          if (++stage == Cfg::kStages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===== consumers: MMA + epilogue =====
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2;   // rows [64 wg, 64 wg + 64) of the tile
+  const uint32_t smem0 = smem_u32(smem);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int m_blk, n_blk;
+    tile_to_mn(ea_gm, tile, num_m, num_n, m_blk, n_blk);
+    const int row0 = m_blk * kBlockM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    QkvRowMeta rm[2];
+    if constexpr (EPI == EPI_QKV_ROPE) {   // overlaps the mainloop's loads
+      qkv_row_meta(ea, row0, row0 < M, rm[0]);
+      qkv_row_meta(ea, row0 + 8, row0 + 8 < M, rm[1]);
+    }
+    float acc[BLOCK_N / 2];
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < num_k; ++kb) {
+      mbar_wait(smem_u32(&full_bar[stage]), phase);
+      const uint32_t sa = smem0 + stage * Cfg::kStageBytes + wg * 64 * 128;
+      const uint32_t sb = smem0 + stage * Cfg::kStageBytes + Cfg::kABytes;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockK / 16; ++k)
+        wgmma_ss<BLOCK_N>(acc, gmma_desc_k_sw128(sa + 32 * k), gmma_desc_k_sw128(sb + 32 * k));
+      wgmma_commit();
+      // the previous K block has retired once at most this one is in flight: free its stage
+      wgmma_wait<1>();
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+      }
+      prev = stage;
+      if (++stage == Cfg::kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+    }
+    if constexpr (EPI == EPI_QKV_ROPE) {
+      static_assert(BLOCK_N % 128 == 0 || EPI != EPI_QKV_ROPE, "fused QKV needs whole heads");
+#pragma unroll
+      for (int hh = 0; hh < BLOCK_N / 128; ++hh) {
+        const int head = (n_blk * BLOCK_N) / kHeadDim + hh;
+        qkv_head_epilogue(acc, hh, ea, rm, row0, M, head, head * kHeadDim < N,
+                          reinterpret_cast<__nv_bfloat16*>(d_out), ldd);
+      }
+    } else {
+      epilogue_store<BLOCK_N, EPI>(acc, d_out, resid, row0, n_blk * BLOCK_N + 2 * (lane & 3), M,
+                                   N, ldd);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------
+// host side: tensor maps
+// ---------------------------------------------------------------------------
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
+                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
+                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+EncodeTiledFn get_encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) ==
+            cudaSuccess &&
+        qres == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+  });
+  return fn;
+}
+
+struct TmapKey {
+  const void* ptr;
+  int rows, cols, box_rows;
+  bool operator==(const TmapKey& o) const {
+    return ptr == o.ptr && rows == o.rows && cols == o.cols && box_rows == o.box_rows;
+  }
+};
+struct TmapKeyHash {
+  size_t operator()(const TmapKey& k) const {
+    size_t h = reinterpret_cast<size_t>(k.ptr);
+    h ^= (static_cast<size_t>(k.rows) * 0x9E3779B97F4A7C15ull) ^
+         (static_cast<size_t>(k.cols) << 20) ^ (static_cast<size_t>(k.box_rows) << 50);
+    return h;
+  }
+};
+
+// Row-major bf16 [rows, cols] tensor, box = [box_rows, 64 cols], 128B swizzle.
+int make_tmap(const void* ptr, int rows, int cols, int box_rows, CUtensorMap* out) {
+  static std::mutex mu;
+  static std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> cache;
+  TmapKey key{ptr, rows, cols, box_rows};
+  {
+    std::lock_guard<std::mutex> g(mu);
+    auto it = cache.find(key);
+    if (it != cache.end()) {
+      *out = it->second;
+      return 0;
+    }
+  }
+  EncodeTiledFn enc = get_encode_fn();
+  if (!enc) {
+    set_last_error("cuTensorMapEncodeTiled entry point unavailable");
+    return -1;
+  }
+  cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(cols) * 2};
+  cuuint32_t box[2] = {static_cast<cuuint32_t>(kBlockK), static_cast<cuuint32_t>(box_rows)};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides,
+                   box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("cuTensorMapEncodeTiled failed: %d (ptr=%p rows=%d cols=%d box_rows=%d)",
+                   static_cast<int>(r), ptr, rows, cols, box_rows);
+    return -1;
+  }
+  std::lock_guard<std::mutex> g(mu);
+  cache.emplace(key, *out);
+  return 0;
+}
+
+}  // namespace
+
+// Generic bf16 tiled tensor map with 128-byte swizzle (rank 2..5); strides are in bytes for
+// dims 1..rank-1 (dim 0 is contiguous).  Used by the attention kernels.
+int encode_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims,
+                     const uint64_t* strides_bytes, const uint32_t* box) {
+  EncodeTiledFn enc = get_encode_fn();
+  if (!enc) {
+    set_last_error("cuTensorMapEncodeTiled entry point unavailable");
+    return -1;
+  }
+  cuuint64_t d[5], st[4];
+  cuuint32_t bx[5], es[5];
+  for (int i = 0; i < rank; ++i) {
+    d[i] = dims[i];
+    bx[i] = box[i];
+    es[i] = 1;
+    if (i + 1 < rank) st[i] = strides_bytes[i];
+  }
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, static_cast<cuuint32_t>(rank),
+                   const_cast<void*>(ptr), d, st, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("cuTensorMapEncodeTiled(rank %d) failed: %d (ptr=%p dims=%llu,%llu box=%u,%u)",
+                   rank, static_cast<int>(r), ptr, (unsigned long long)dims[0],
+                   (unsigned long long)dims[1], box[0], box[1]);
+    return -1;
+  }
+  return 0;
+}
+
+namespace {
+
+int num_sms() {
+  static int cached[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64) dev = 0;
+  if (cached[dev] == 0) {
+    int n = 0;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    cached[dev] = n > 0 ? n : 1;
+  }
+  return cached[dev];
+}
+
+int l2_bytes() {
+  static long cached = -1;
+  if (cached < 0) {
+    int dev = 0, n = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrL2CacheSize, dev);
+    cached = n > 0 ? n : (40 << 20);
+  }
+  return static_cast<int>(cached);
+}
+
+// Row-tiles per raster group.  A weight matrix that fits in half the L2 (QKV, Wo, down of the
+// smaller models) stays resident whatever the order, so narrow groups are enough: the CTAs of a
+// wave then share few A row-tiles and walk W together.  A larger W (gate/up, the LM head) is
+// streamed: there the group takes as many row-tiles as keep its A slab (rows x K bf16) within
+// ~40 % of the L2, so A is read from HBM once and W once per group.
+int raster_group(int tile_rows, int N, int K) {
+  static const int forced = [] {   // SB200_GEMM_GM: fixes the group size (tuning experiments)
+    const char* e = getenv("SB200_GEMM_GM");
+    return e ? atoi(e) : 0;
+  }();
+  if (forced > 0) return forced;
+  const long l2 = l2_bytes();
+  if (static_cast<long>(N) * K * 2 <= l2 / 2) return 2;
+  const long slab = l2 * 2 / 5;
+  long gm = slab / (static_cast<long>(tile_rows) * K * 2);
+  if (gm < 2) gm = 2;
+  if (gm > 64) gm = 64;
+  return static_cast<int>(gm);
+}
+
+template <int BLOCK_N, int EPI>
+int launch_cfg(const void* a, int a_rows, const void* w, void* d, const void* resid, int M, int N,
+               int K, int ldd, cudaStream_t stream, const QkvEpiArgs& ea) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  CUtensorMap tm_a, tm_b;
+  if (make_tmap(a, a_rows, K, kBlockM, &tm_a)) return -1;
+  if (make_tmap(w, N, K, BLOCK_N, &tm_b)) return -1;
+  auto kern = gemm_bf16_tn_kernel<BLOCK_N, EPI>;
+  SB_SET_MAX_SMEM(kern, Cfg::kSmemBytes);
+  const int tiles = ((M + kBlockM - 1) / kBlockM) * ((N + BLOCK_N - 1) / BLOCK_N);
+  const int grid = tiles < num_sms() ? tiles : num_sms();
+  kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(
+      tm_a, tm_b, d, reinterpret_cast<const __nv_bfloat16*>(resid), M, N, K, ldd,
+      raster_group(kBlockM, N, K), ea);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
+template <int EPI>
+int launch_epi(int block_n, const void* a, int a_rows, const void* w, void* d, const void* resid,
+               int M, int N, int K, int ldd, cudaStream_t stream, const QkvEpiArgs& ea) {
+  switch (block_n) {
+    case 64:
+      if constexpr (EPI == EPI_QKV_ROPE) {
+        set_last_error("gemm_bf16_tn: the fused QKV epilogue needs block_n >= 128");
+        return -1;
+      } else {
+        return launch_cfg<64, EPI>(a, a_rows, w, d, resid, M, N, K, ldd, stream, ea);
+      }
+    case 128:
+      return launch_cfg<128, EPI>(a, a_rows, w, d, resid, M, N, K, ldd, stream, ea);
+    default:   // 256, and 512 (the widest tile)
+      return launch_cfg<256, EPI>(a, a_rows, w, d, resid, M, N, K, ldd, stream, ea);
+  }
+}
+
+}  // namespace
+
+int gemm_pick_block_n(int M, int N) {
+  // Cost = waves x (tile area / efficiency); pick the cheapest configuration (one CTA per SM,
+  // 128 x BLOCK_N tiles).  The relative efficiencies are assumed, not measured: a narrow tile
+  // moves more operand bytes per MAC, (128 + BLOCK_N) / (128 * BLOCK_N), which alone would rate
+  // the 128- and 64-wide tiles at 0.75 / 0.5 of the 256-wide one; they are rated higher because
+  // shared-memory traffic is not the only limit.  Every tile width accumulates in the same order,
+  // so the choice changes speed only, never results.
+  const int sms = num_sms();
+  double best = 1e30;
+  int pick = 128;
+  struct Cand { int tn; double eff; };
+  const Cand cands[] = {{256, 1.0}, {128, 0.85}, {64, 0.6}};
+  for (const Cand& c : cands) {
+    const long tiles = static_cast<long>((M + kBlockM - 1) / kBlockM) * ((N + c.tn - 1) / c.tn);
+    const long waves = (tiles + sms - 1) / sms;
+    const double cost = static_cast<double>(waves) * kBlockM * c.tn / c.eff;
+    if (cost < best) {
+      best = cost;
+      pick = c.tn;
+    }
+  }
+  return pick;
+}
+
+int gemm_bf16_tn(const void* a, int a_rows, const void* w, void* d, const void* resid, int M,
+                 int N, int K, int ldd, int epilogue, int block_n, cudaStream_t stream,
+                 const QkvEpiArgs* qkv_args) {
+  if (M <= 0) return 0;
+  const QkvEpiArgs ea = qkv_args ? *qkv_args : QkvEpiArgs{};
+  if (K % kBlockK != 0 || N % 32 != 0 || a_rows < M) {
+    set_last_error("gemm_bf16_tn: unsupported shape M=%d N=%d K=%d a_rows=%d", M, N, K, a_rows);
+    return -1;
+  }
+  if (block_n == 0) block_n = gemm_pick_block_n(M, N);
+  if (block_n != 64 && block_n != 128 && block_n != 256 && block_n != 512) {
+    set_last_error("gemm_bf16_tn: block_n must be 64/128/256/512, got %d", block_n);
+    return -1;
+  }
+  switch (epilogue) {
+    case EPI_STORE_BF16:
+      return launch_epi<EPI_STORE_BF16>(block_n, a, a_rows, w, d, resid, M, N, K, ldd, stream, ea);
+    case EPI_RESIDUAL_BF16:
+      if (!resid) {
+        set_last_error("gemm_bf16_tn: residual epilogue without residual pointer");
+        return -1;
+      }
+      return launch_epi<EPI_RESIDUAL_BF16>(block_n, a, a_rows, w, d, resid, M, N, K, ldd, stream, ea);
+    case EPI_SWIGLU_BF16:
+      return launch_epi<EPI_SWIGLU_BF16>(block_n, a, a_rows, w, d, resid, M, N, K, ldd, stream, ea);
+    case EPI_STORE_F32:
+      return launch_epi<EPI_STORE_F32>(block_n, a, a_rows, w, d, resid, M, N, K, ldd, stream, ea);
+    case EPI_QKV_ROPE:
+      if (!qkv_args || N % kHeadDim != 0 || N != (ea.hq + 2 * ea.hkv) * kHeadDim) {
+        set_last_error("gemm_bf16_tn: fused QKV epilogue needs its operands and N = heads*128");
+        return -1;
+      }
+      if (block_n == 64) block_n = 128;
+      return launch_epi<EPI_QKV_ROPE>(block_n, a, a_rows, w, d, resid, M, N, K, ldd, stream, ea);
+    default:
+      set_last_error("gemm_bf16_tn: unknown epilogue %d", epilogue);
+      return -1;
+  }
+}
+
+}  // namespace sb

@@ -88,7 +88,7 @@ int attn_prefill(const void* qkv, void* out, const void* kv_layer, const int32_t
                  int hq, int hkv, float scale, cudaStream_t stream);
 int attn_prefill_q_tile(int hq, int hkv);
 
-// K3 (tcgen05) — causal prefill attention over DENSE K/V: new tokens' K/V are the k/v columns
+// K3 (wgmma) — causal prefill attention over DENSE K/V: new tokens' K/V are the k/v columns
 // of the qkv buffer itself (post-norm/RoPE, written by the fused QKV epilogue), the shared
 // prefix's K/V live in prefix_kv[n_layers][prefix_rows][2*hkv*128] (K heads | V heads).
 // items: [n_items] {seq, q_tile_start} with q tile = attn_prefill_q_tile(); every sequence
@@ -98,7 +98,7 @@ int attn_prefill_dense(const void* qkv, int t_rows, void* out, const void* prefi
                        const int32_t* seq_q_start, const int32_t* seq_q_len,
                        const int32_t* seq_past, int hq, int hkv, float scale, cudaStream_t stream);
 
-// bf16 tensor map, 128-byte swizzle, rank 2..5 (gemm_tcgen05.cu)
+// bf16 tensor map, 128-byte swizzle, rank 2..5 (gemm_wgmma.cu)
 int encode_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims,
                      const uint64_t* strides_bytes, const uint32_t* box);
 

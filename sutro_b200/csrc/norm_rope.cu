@@ -211,7 +211,7 @@ rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __restrict_
       const int within = (4 * l) & 7;      // 0 or 4 elements into the chunk
       *reinterpret_cast<uint2*>(tile + ((c_lo ^ (r & 7)) << 3) + within) = plo;
       *reinterpret_cast<uint2*>(tile + ((c_hi ^ (r & 7)) << 3) + within) = phi;
-      if (is_k) {  // dense copy for the tcgen05 prefill attention (V is already in place)
+      if (is_k) {  // dense copy for the wgmma prefill attention (V is already in place)
         *reinterpret_cast<uint2*>(hp + 4 * l) = plo;
         *reinterpret_cast<uint2*>(hp + 64 + 4 * l) = phi;
       }

@@ -328,7 +328,7 @@ class LocalEngine:
                  kv_fraction: float = 0.8, logit_chunk_rows: int = 1024,
                  min_admit_rows: Optional[int] = None):
         if not torch.cuda.is_available():
-            raise L.Sb200Error("sutro_b200 needs a CUDA device (sm_100a); there is no CPU path")
+            raise L.Sb200Error("sutro_b200 needs a CUDA device (sm_90a); there is no CPU path")
         self.device = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
         self.spec, self.weights, self.vocab = spec, weights, vocab
         if vocab.vocab_size != spec.vocab_size:

@@ -1,4 +1,4 @@
-"""`Sutro` — the local, B200-native counterpart of the reference SDK client for the
+"""`Sutro` — the local, H100-native counterpart of the reference SDK client for the
 infer() hot path (reference: sutro/sdk.py:46, `class Sutro`).
 
 Drop-in surface (same names, positional order, defaults, return and error
@@ -11,7 +11,7 @@ conventions as the reference):
 What changes is what happens at the reference's single process boundary
 (`do_request("POST", "batch-inference")`, sutro/sdk.py:223): instead of shipping the
 column to a hosted service, the rows go through `engine.LocalEngine.generate` on this
-machine's B200(s).  Jobs complete before infer() returns, so the polling helpers
+machine's H100(s).  Jobs complete before infer() returns, so the polling helpers
 resolve immediately; results are kept in memory and (like the reference,
 sutro/sdk.py:1065-1117) cached as snappy parquet under ~/.sutro/job-results/.
 
@@ -382,7 +382,7 @@ class Sutro(Templates, BaseSutroClient):
         random_seed_per_input: bool = False,
         truncate_rows: bool = True,
     ):
-        """Run inference over `data` on the local B200 engine; returns the job id."""
+        """Run inference over `data` on the local H100 engine; returns the job id."""
         model = self._resolve_model(model)
         if stay_attached is None:
             stay_attached = job_priority == 0

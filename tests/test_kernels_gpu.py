@@ -42,7 +42,7 @@ def _gemm(a, w, epi=0, resid=None, block_n=0, m=None, out=None):
     return out
 
 
-@pytest.mark.parametrize("block_n", [64, 128, 256, 512, 0])  # 512 = CTA-pair kernel
+@pytest.mark.parametrize("block_n", [64, 128, 256, 512, 0])  # 512 = the widest tile
 @pytest.mark.parametrize("M,N,K", [(128, 256, 64), (128, 256, 256), (300, 768, 512),
                                    (1000, 1536, 2560), (77, 32 * 11, 192)])
 def test_gemm_store_bf16(M, N, K, block_n):
@@ -82,7 +82,7 @@ def test_gemm_exact_integers_at_the_benchmark_shapes(M, N, K, epi):
     """The shapes that earn the roofline number (multi-group raster, many waves, K up to
     9728), on small-integer operands: every partial sum is exact in fp32, so the kernel must
     agree BIT FOR BIT with a plain fp32 matmul (+ the documented bf16 rounding points),
-    whatever tile shape, raster order or CTA pairing the launcher picked."""
+    whatever tile shape or raster order the launcher picked."""
     torch.manual_seed(M + N + K)
     a = bf(torch.randint(-2, 3, (M, K), device=DEV).float())
     w = bf(torch.randint(-2, 3, (N, K), device=DEV).float())
@@ -115,8 +115,8 @@ def test_gemm_swiglu_at_the_benchmark_shape():
 
 def test_gemm_tile_configurations_are_bit_identical():
     """Batch invariance of the GEMM: the launcher picks the tile shape from M (128x64 ...
-    256x256 CTA pair), so a row's result must not depend on that choice — every configuration
-    accumulates over K in the same order (k-blocks of 64, four K=16 UMMA steps each)."""
+    128x256), so a row's result must not depend on that choice — every configuration
+    accumulates over K in the same order (k-blocks of 64, four K=16 wgmma steps each)."""
     torch.manual_seed(21)
     M, N, K = 300, 1536, 2560
     a = bf(torch.randn(M, K, device=DEV))
@@ -146,7 +146,7 @@ def test_gemm_a_rows_larger_than_m():
 
 @pytest.mark.parametrize("epi", [1, 2])
 def test_gemm_cta_pair_fused_epilogues(epi):
-    """residual / SwiGLU epilogues through the cta_group::2 kernel at a multi-wave shape."""
+    """residual / SwiGLU epilogues through the widest tile at a multi-wave shape."""
     M, N, K = 1500, 5120, 1024
     torch.manual_seed(7)
     a = bf(torch.randn(M, K, device=DEV))
@@ -469,8 +469,8 @@ def _dense_ref(qkv, pre, layer, hq, hkv, specs, q_start, scale):
 
 @pytest.mark.parametrize("hq,hkv", [(32, 8), (16, 8), (4, 4), (16, 2)])
 def test_attn_prefill_dense_tcgen05(hq, hkv):
-    """K3 on tcgen05: new tokens attend to [dense shared prefix | own rows] (TMA-fed UMMA,
-    S/O in TMEM) — against an fp32 softmax(QK^T)V over the same bf16 inputs."""
+    """K3 on wgmma: new tokens attend to [dense shared prefix | own rows] (TMA-fed wgmma,
+    S/O in registers) — against an fp32 softmax(QK^T)V over the same bf16 inputs."""
     specs = [(0, 1), (0, 16), (0, 17), (0, 100), (32, 5), (32, 70), (48, 200), (3, 33),
              (46, 111), (130, 140), (200, 300), (0, 129), (1, 128)]
     n_layers, layer, prefix_rows = 3, 1, 200
@@ -493,8 +493,8 @@ def test_attn_prefill_dense_tcgen05(hq, hkv):
 
 
 def test_attn_prefill_dense_rescale_and_no_prefix():
-    """Large score magnitudes force the lazy running-max rescale of the TMEM accumulator
-    (O is rewritten through tcgen05.ld/st); prefix_kv may be NULL when nothing has a past."""
+    """Large score magnitudes force the lazy running-max rescale of the register
+    accumulator O; prefix_kv may be NULL when nothing has a past."""
     hq, hkv = 8, 2
     specs = [(0, 700), (0, 260), (0, 31)]
     qkv, pre, q_start, items, T = _dense_case(hq, hkv, specs, 0, 1, 0, seed=3, q_gain=6.0)

@@ -74,10 +74,54 @@ SB_DEVICE void tile_to_mn(int GM, int tile, int num_m, int num_n, int& m_blk, in
 
 // This thread's accumulators (rows row0 and row0 + 8, columns col0 + 8j + {0, 1}) -> fused
 // epilogue -> global.  col0 already includes the lane's 2 * (lane % 4).
+// RESIDUAL_BF16: D = bf16(bf16(acc) + R), R read from HBM.  Loaded one element pair before
+// its store, as the compiler schedules a plain loop, only a few loads are in flight per thread
+// and the epilogue becomes a chain of memory round trips that kept the tensor cores idle for
+// longer than the mainloop of a K = 4096 tile (O-projection at 0.35 of the rate of the same
+// GEMM with a plain bf16 store).  So the loads of a chunk of kChunk column groups are issued
+// together, then the chunk is rounded, summed and stored: four round trips per 256-wide tile.
+// A chunk of 16 spills: ptxas allots 168 registers, 128 of them accumulators.
+template <int BLOCK_N>
+SB_DEVICE void epilogue_residual(const float (&acc)[BLOCK_N / 2], __nv_bfloat16* d_out,
+                                 const __nv_bfloat16* resid, int row0, int col0, int M, int N,
+                                 int ldd) {
+  constexpr int kChunk = 8;
+#pragma unroll
+  for (int j0 = 0; j0 < BLOCK_N / 8; j0 += kChunk) {
+    uint32_t r[kChunk][2];
+#pragma unroll
+    for (int j = 0; j < kChunk; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int col = col0 + 8 * (j0 + j), row = row0 + 8 * h;
+        // volatile: the compiler would otherwise sink each load to its use again
+        asm volatile(
+            "{\n.reg .pred p;\nsetp.ne.b32 p, %2, 0;\nmov.b32 %0, 0;\n"
+            "@p ld.global.b32 %0, [%1];\n}\n"
+            : "=r"(r[j][h])
+            : "l"(resid + static_cast<size_t>(row) * ldd + col), "r"(int(col < N && row < M)));
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < kChunk; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int col = col0 + 8 * (j0 + j), row = row0 + 8 * h;
+        if (col < N && row < M) {
+          const float2 rv = unpack_bf16x2(r[j][h]);
+          const int i = 4 * (j0 + j) + 2 * h;
+          *reinterpret_cast<uint32_t*>(d_out + static_cast<size_t>(row) * ldd + col) =
+              pack_bf16x2(bf16_round(acc[i]) + rv.x, bf16_round(acc[i + 1]) + rv.y);
+        }
+      }
+    }
+  }
+}
+
+// STORE_BF16, SWIGLU_BF16, STORE_F32.
 template <int BLOCK_N, int EPI>
 SB_DEVICE void epilogue_store(const float (&acc)[BLOCK_N / 2], void* __restrict__ d_out,
-                              const __nv_bfloat16* __restrict__ resid, int row0, int col0, int M,
-                              int N, int ldd) {
+                              int row0, int col0, int M, int N, int ldd) {
   const int lane = threadIdx.x & 31;
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j) {
@@ -102,10 +146,6 @@ SB_DEVICE void epilogue_store(const float (&acc)[BLOCK_N / 2], void* __restrict_
       } else if (ok) {
         if constexpr (EPI == EPI_STORE_F32) {
           *reinterpret_cast<float2*>(reinterpret_cast<float*>(d_out) + off) = make_float2(v0, v1);
-        } else if constexpr (EPI == EPI_RESIDUAL_BF16) {
-          const float2 r = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(resid + off));
-          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(d_out) + off) =
-              pack_bf16x2(bf16_round(v0) + r.x, bf16_round(v1) + r.y);
         } else {
           *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(d_out) + off) =
               pack_bf16x2(v0, v1);
@@ -346,9 +386,13 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
         qkv_head_epilogue(acc, hh, ea, rm, row0, M, head, head * kHeadDim < N,
                           reinterpret_cast<__nv_bfloat16*>(d_out), ldd);
       }
+    } else if constexpr (EPI == EPI_RESIDUAL_BF16) {
+      // in place (resid == d_out) in the engine: each element is read before it is written,
+      // by the same thread
+      epilogue_residual<BLOCK_N>(acc, reinterpret_cast<__nv_bfloat16*>(d_out), resid, row0,
+                                 n_blk * BLOCK_N + 2 * (lane & 3), M, N, ldd);
     } else {
-      epilogue_store<BLOCK_N, EPI>(acc, d_out, resid, row0, n_blk * BLOCK_N + 2 * (lane & 3), M,
-                                   N, ldd);
+      epilogue_store<BLOCK_N, EPI>(acc, d_out, row0, n_blk * BLOCK_N + 2 * (lane & 3), M, N, ldd);
     }
   }
 }

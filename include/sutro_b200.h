@@ -52,7 +52,9 @@ int sb200_gemm_bf16_tn(const void* a, int a_rows, const void* w, void* d, const 
 
 /* K1+K5 fused: qkv = A Wqkv^T with per-head q/k RMSNorm + RoPE + paged K/V write applied in
  * the GEMM epilogue (same result as sb200_gemm_bf16_tn followed by sb200_rope_kv_write);
- * q heads land in qkv_out[:, :hq*128], K/V go straight to the cache.  block_n: 0/128/256/512. */
+ * q heads land in qkv_out[:, :hq*128]; the post-norm/RoPE K and the V go to the paged cache AND,
+ * unswizzled and bit-identical, to their columns of qkv_out (the dense copy that
+ * sb200_attn_prefill_dense reads).  Rows >= M of qkv_out are not written.  block_n: 0/128/256/512. */
 int sb200_gemm_qkv_rope(const void* a, int a_rows, const void* w, void* qkv_out, int M, int K,
                         int block_n, const void* q_norm_w, const void* k_norm_w,
                         const void* cos_tab, const void* sin_tab, const int32_t* tok_slot,
@@ -75,7 +77,10 @@ int sb200_rope_kv_write(void* qkv, const void* q_norm_w, const void* k_norm_w, c
                         const int32_t* page_table, int max_pages, void* kv_layer, int T, int hq,
                         int hkv, float eps, void* stream);
 
-/* K2: paged-KV decode attention, one query token per sequence. */
+/* K2: paged-KV decode attention, one query token per sequence.  Whole 16-token pages are loaded:
+ * the V values of the slots at or after ctx_len in a sequence's last page must be finite (0 * NaN
+ * would reach the output); their K values are never used.  Page-table entries past a sequence's
+ * last page are not read. */
 int sb200_attn_decode(const void* qkv, void* out, const void* kv_layer, const int32_t* page_table,
                       int max_pages, const int32_t* row_slot, const int32_t* ctx_len, int B, int hq,
                       int hkv, float scale, void* stream);
@@ -83,7 +88,8 @@ int sb200_attn_decode(const void* qkv, void* out, const void* kv_layer, const in
 /* test hook: 0 = automatic choice, 1 = 4-warps-per-pair split kernel, 2 = warp-per-pair */
 void sb200_attn_decode_force_variant(int v);
 
-/* K3: causal varlen prefill attention over the paged cache. */
+/* K3: causal varlen prefill attention over the paged cache.  As for decode, the V values of the
+ * slots past a sequence's last token in its last page must be finite. */
 int sb200_attn_prefill(const void* qkv, void* out, const void* kv_layer, const int32_t* page_table,
                        int max_pages, const int32_t* work, int n_work, const int32_t* seq_slot,
                        const int32_t* seq_q_start, const int32_t* seq_q_len,

@@ -21,7 +21,8 @@
 //   SWIGLU_BF16    D[:, j] = bf16(silu(bf16(acc[2j])) * bf16(acc[2j+1]))
 //                  (gate/up weights interleaved row-wise; output has N/2 columns)
 //   STORE_F32      D = acc                             (lm_head logits)
-//   QKV_ROPE       q/k RMSNorm + RoPE, K/V into the paged cache (see qkv_head_epilogue)
+//   QKV_ROPE       q/k RMSNorm + RoPE, K/V into the paged cache and into their columns of D
+//                  (the dense copy the prefill attention reads; see qkv_head_epilogue)
 #include <algorithm>
 #include <cstdlib>
 #include <mutex>

@@ -10,6 +10,7 @@ import torch
 
 from sutro_b200 import _lib as L
 import kv_layout as KV
+from test_attention_exact_gpu import assert_within_bound, attn_ref64
 
 pytestmark = pytest.mark.gpu
 
@@ -353,17 +354,6 @@ def test_gemm_qkv_rope_fused_matches_unfused(qk_norm, block_n):
 
 
 # --------------------------------------------------------------------------- attention
-def attn_ref(q, k, v, scale):
-    """q: [hq,128], k/v: [L,hkv,128] -> [hq,128]; fp32 softmax, bf16 P (like the kernel)."""
-    hq, hkv = q.shape[0], k.shape[1]
-    g = hq // hkv
-    kk = k.float().repeat_interleave(g, dim=1)  # [L,hq,128]
-    vv = v.float().repeat_interleave(g, dim=1)
-    s = torch.einsum("hd,lhd->hl", q.float(), kk) * scale
-    p = torch.softmax(s, dim=-1)
-    return torch.einsum("hl,lhd->hd", p, vv)
-
-
 @pytest.mark.parametrize("variant", [1, 2])   # 1: 4-warp split kernel, 2: warp-per-pair kernel
 @pytest.mark.parametrize("hq,hkv", [(32, 8), (16, 8), (8, 8), (16, 2)])
 def test_attn_decode(hq, hkv, variant):
@@ -384,12 +374,10 @@ def test_attn_decode(hq, hkv, variant):
                                       L.ptr(row_slot), L.ptr(ctx), B, hq, hkv, scale, stream()))
     torch.cuda.synchronize()
     L.lib().sb200_attn_decode_force_variant(0)
-    for b in range(B):
-        s = B - 1 - b
-        q = qkv[b].view(hq + 2 * hkv, KV.HD)[:hq]
-        ref = attn_ref(q, ks[s], vs[s], scale)
-        got = out[b].view(hq, KV.HD).float()
-        assert torch.allclose(got, ref, rtol=2e-2, atol=2e-2), (b, (got - ref).abs().max())
+    refs = [attn_ref64(qkv[b:b + 1, :hq * KV.HD].view(1, hq, KV.HD), ks[B - 1 - b], vs[B - 1 - b],
+                       [lens[B - 1 - b]], hkv) for b in range(B)]
+    assert_within_bound(out, torch.cat([r for r, _ in refs]), torch.cat([m for _, m in refs]),
+                        f"decode variant {variant} {hq}/{hkv}")
 
 
 @pytest.mark.parametrize("hq,hkv", [(32, 8), (16, 8), (4, 4)])
@@ -421,13 +409,10 @@ def test_attn_prefill(hq, hkv):
         len(work) // 2, L.ptr(d_slot), L.ptr(d_qs), L.ptr(d_ql), L.ptr(d_past), hq, hkv, scale,
         stream()))
     torch.cuda.synchronize()
-    for i, (p, q) in enumerate(specs):
-        for j in range(q):
-            t = q_start[i] + j
-            qv = qkv[t].view(hq + 2 * hkv, KV.HD)[:hq]
-            ref = attn_ref(qv, ks[i][: p + j + 1], vs[i][: p + j + 1], scale)
-            got = out[t].view(hq, KV.HD).float()
-            assert torch.allclose(got, ref, rtol=2e-2, atol=2e-2), (i, j, (got - ref).abs().max())
+    refs = [attn_ref64(qkv[q_start[i]:q_start[i] + q, :hq * KV.HD].view(q, hq, KV.HD), ks[i],
+                       vs[i], p + 1 + torch.arange(q), hkv) for i, (p, q) in enumerate(specs)]
+    assert_within_bound(out, torch.cat([r for r, _ in refs]), torch.cat([m for _, m in refs]),
+                        f"paged prefill {hq}/{hkv}")
 
 
 def _dense_case(hq, hkv, specs, prefix_rows, n_layers, layer, seed, q_gain=1.0, t_pad=7):
@@ -449,22 +434,16 @@ def _dense_case(hq, hkv, specs, prefix_rows, n_layers, layer, seed, q_gain=1.0, 
     return qkv, pre, q_start, items, T
 
 
-def _dense_ref(qkv, pre, layer, hq, hkv, specs, q_start, scale):
-    """fp32 reference of the dense prefill attention: [T, hq, 128]."""
-    out = []
+def _dense_ref(qkv, pre, layer, hq, hkv, specs, q_start):
+    """fp64 reference of the dense prefill attention: (ref, mag) [T, hq, 128] (see
+    test_attention_exact_gpu.error_bound)."""
+    refs = []
     for i, (p, q) in enumerate(specs):
         rows = qkv[q_start[i]:q_start[i] + q].view(q, hq + 2 * hkv, KV.HD)
-        kown, vown = rows[:, hq:hq + hkv], rows[:, hq + hkv:]
-        pk = pre[layer, :p, :hkv * KV.HD].view(p, hkv, KV.HD)
-        pv = pre[layer, :p, hkv * KV.HD:].view(p, hkv, KV.HD)
-        k = torch.cat([pk, kown]).float().repeat_interleave(hq // hkv, dim=1)   # [p+q, hq, 128]
-        v = torch.cat([pv, vown]).float().repeat_interleave(hq // hkv, dim=1)
-        s = torch.einsum("qhd,lhd->hql", rows[:, :hq].float(), k) * scale       # [hq, q, p+q]
-        pos_q = torch.arange(q, device=DEV)[:, None] + p
-        pos_k = torch.arange(p + q, device=DEV)[None, :]
-        s = s.masked_fill(pos_k > pos_q, float("-inf"))
-        out.append(torch.einsum("hql,lhd->qhd", torch.softmax(s, dim=-1), v))
-    return torch.cat(out)
+        k = torch.cat([pre[layer, :p, :hkv * KV.HD].view(p, hkv, KV.HD), rows[:, hq:hq + hkv]])
+        v = torch.cat([pre[layer, :p, hkv * KV.HD:].view(p, hkv, KV.HD), rows[:, hq + hkv:]])
+        refs.append(attn_ref64(rows[:, :hq], k, v, p + 1 + torch.arange(q), hkv))
+    return torch.cat([r for r, _ in refs]), torch.cat([m for _, m in refs])
 
 
 @pytest.mark.parametrize("hq,hkv", [(32, 8), (16, 8), (4, 4), (16, 2)])
@@ -486,10 +465,8 @@ def test_attn_prefill_dense_tcgen05(hq, hkv):
         L.ptr(d_items), len(items) // 2, L.ptr(d_qs), L.ptr(d_ql), L.ptr(d_past), hq, hkv, scale,
         stream()))
     torch.cuda.synchronize()
-    ref = _dense_ref(qkv, pre, layer, hq, hkv, specs, q_start, scale)
-    got = out.view(T, hq, KV.HD).float()
-    err = (got - ref).abs()
-    assert torch.allclose(got, ref, rtol=2e-2, atol=2e-2), (err.max(), err.argmax())
+    ref, mag = _dense_ref(qkv, pre, layer, hq, hkv, specs, q_start)
+    assert_within_bound(out, ref, mag, f"dense prefill {hq}/{hkv}")
 
 
 def test_attn_prefill_dense_rescale_and_no_prefix():
@@ -507,9 +484,8 @@ def test_attn_prefill_dense_rescale_and_no_prefix():
         L.ptr(qkv), qkv.shape[0], L.ptr(out), None, 0, 1, 0, L.ptr(d_items), len(items) // 2,
         L.ptr(d_qs), L.ptr(d_ql), L.ptr(d_past), hq, hkv, scale, stream()))
     torch.cuda.synchronize()
-    ref = _dense_ref(qkv, pre, 0, hq, hkv, specs, q_start, scale)
-    got = out.view(T, hq, KV.HD).float()
-    assert torch.allclose(got, ref, rtol=3e-2, atol=3e-2), (got - ref).abs().max()
+    ref, mag = _dense_ref(qkv, pre, 0, hq, hkv, specs, q_start)
+    assert_within_bound(out, ref, mag, "dense prefill, q_gain 6")
 
 
 def test_attn_prefill_dense_is_batch_invariant():

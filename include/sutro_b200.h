@@ -114,6 +114,53 @@ int sb200_fsm_build_mask(const int32_t* fsm_trans, const uint8_t* fsm_accept, in
                          const uint8_t* tok_bytes, const int32_t* tok_off, int vocab, int eos_id,
                          uint32_t* mask_bits, int mask_words, void* stream);
 
+/* Test hook: one sampling step (K8) exactly as the engine runs it on a chunk of logits rows.
+ * The fields mirror the engine's internal arguments one for one; every pointer is a device
+ * pointer.  Values are used as given: temperature <= 0 runs the greedy kernel (arg-max, lowest
+ * index wins ties), top_k <= 0 and top_p >= 1 switch those filters off (the engine's
+ * "top_p = 0 means off" is not applied here).  Rows whose slot is done are skipped.
+ * out_tau (optional, [B]): for every row the stochastic kernel samples, the order-preserving
+ * key of the smallest kept z = logit * (1/T): bits of z with the sign bit set when z >= 0, all
+ * bits inverted when z < 0, -0.0 taken as +0.0; 0 when no filter is active.  The kept set is
+ * then exactly {allowed i : key(z_i) >= out_tau}.  Not written by the greedy kernel, nor for
+ * rows where nothing is selectable. */
+typedef struct {
+  const float* logits;      /* [B, ldl] fp32                                                */
+  int ldl, vocab, B;
+  const int32_t* row_slot;  /* [B] slot of each logits row                                  */
+  int32_t* slot_state;      /* per slot: DFA state, -1 = unconstrained (NULL = all -1)      */
+  int32_t* slot_ngen;       /* tokens generated so far (Philox step counter)                */
+  int32_t* slot_next_tok;   /* out: the sampled token                                       */
+  int32_t* slot_pos;        /* incremented by one                                           */
+  int32_t* slot_done;       /* set to 1 when the row ends at this step                      */
+  const int32_t* slot_row;  /* output row of each slot                                      */
+  const int32_t* slot_maxnew;
+  int32_t* out_tokens;      /* [n_rows, out_stride]                                         */
+  int32_t* out_len;         /* [n_rows]                                                     */
+  int out_stride;
+  const uint32_t* mask_bits; /* [n_states, mask_words] from sb200_fsm_build_mask, or NULL   */
+  int mask_words;
+  const int32_t* fsm_trans;  /* [n_states, 256], -1 = dead                                  */
+  const uint8_t* fsm_accept;
+  const uint8_t* fsm_final;
+  const int32_t* fsm_tail_off; /* [n_states+1] jump-forward tails, or NULL                  */
+  const int32_t* fsm_tail_tok;
+  const uint8_t* tok_bytes;  /* vocabulary byte strings                                     */
+  const int32_t* tok_off;    /* [vocab+1]                                                   */
+  int eos_id, ignore_eos;
+  float temperature;
+  int top_k;
+  float top_p;
+  uint64_t seed;
+  int seed_per_row;
+  const int64_t* row_ids;    /* optional [n_rows]: Philox stream id per row                 */
+  float* slot_cum_logprob;   /* optional: running sum of log p(token)                       */
+  float* out_cum_logprob;    /* optional [n_rows]                                           */
+  uint32_t* out_tau;         /* optional [B], see above                                     */
+} sb200_sample_args;
+
+int sb200_sample(const sb200_sample_args* args, void* stream);
+
 /* K7: batched byte-level BPE on the GPU.  merges:[n,2] left/right ids in rank order
  * (merged_ids NULL => id 256+rank); cls_table: 0x110000 bytes, Unicode class per code
  * point (0 other, 1 letter, 2 number, 3 white space); digits: max digits per pre-token

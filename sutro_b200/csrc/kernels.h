@@ -141,6 +141,8 @@ struct SampleArgs {
   const int64_t* row_ids;  // optional [n_rows]: stream id per row (null = row index)
   float* slot_cum_logprob; // nullable: running sum of log p(token) under the masked softmax
   float* out_cum_logprob;  // [n_rows], written together with out_len
+  uint32_t* out_tau;       // nullable [B]: order-preserving key of the smallest kept z (stochastic
+                           // kernel only; 0 = no filter).  Kept = allowed and fkey(z) >= tau.
 };
 int sample_greedy(const SampleArgs& a, cudaStream_t stream);  // dispatches on a.temperature
 int prepare_decode(const int32_t* row_slot, const int32_t* slot_next_tok, const int32_t* slot_pos,

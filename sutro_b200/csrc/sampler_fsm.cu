@@ -45,11 +45,13 @@ constexpr int kSampleWarps = kSampleThreads / 32;
 
 // Row bookkeeping shared by the greedy and the stochastic sampler (thread 0 of the CTA):
 // append the token, advance the DFA by its bytes, apply jump-forward tails, raise `done`.
-__device__ void finish_row(const SampleArgs& a, int slot, int state, int tok, float logprob) {
+// `stop`: nothing was selectable; the row ends without output whatever ignore_eos says.
+__device__ void finish_row(const SampleArgs& a, int slot, int state, int tok, float logprob,
+                           bool stop = false) {
   const int row = a.slot_row[slot];
   int ngen = a.slot_ngen[slot];
   bool done = false;
-  if (tok == a.eos_id && !a.ignore_eos) {
+  if (stop || (tok == a.eos_id && !a.ignore_eos)) {
     done = true;
   } else {
     a.out_tokens[static_cast<size_t>(row) * a.out_stride + ngen] = tok;
@@ -134,10 +136,10 @@ __global__ void __launch_bounds__(kSampleThreads) sample_greedy_kernel(SampleArg
     m = better(m, ArgMax{lg[i], i});
   }
   m = block_argmax(m, sv, si);
-  int tok = m.i;
-  if (tok < 0 || tok >= a.vocab) tok = a.eos_id;  // nothing selectable: terminate the row
+  const bool none = m.i < 0 || m.i >= a.vocab;  // nothing selectable: terminate the row
+  const int tok = none ? a.eos_id : m.i;
   float logprob = 0.f;
-  if (a.slot_cum_logprob != nullptr) {  // log-softmax of the masked logits at the arg-max
+  if (a.slot_cum_logprob != nullptr && !none) {  // log-softmax of the masked logits at the arg-max
     float se = 0.f;
     for (int i = threadIdx.x; i < a.vocab; i += kSampleThreads) {
       if (mask && !((mask[i >> 5] >> (i & 31)) & 1u)) continue;
@@ -146,7 +148,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_greedy_kernel(SampleArg
     se = block_sum(se, sv);
     logprob = -__logf(se);
   }
-  if (threadIdx.x == 0) finish_row(a, slot, state, tok, logprob);
+  if (threadIdx.x == 0) finish_row(a, slot, state, tok, logprob, none);
 }
 
 // ---------------------------------------------------------------------------
@@ -157,8 +159,10 @@ __global__ void __launch_bounds__(kSampleThreads) sample_greedy_kernel(SampleArg
 // inverse CDF over the kept set in vocabulary order with one Philox4x32-10 draw per
 // (seed, row, step).
 // ---------------------------------------------------------------------------
+// Order-preserving key of a float.  -0.0 is mapped to +0.0 first: they compare equal, so a
+// tie at zero must give one key or a threshold at +0.0 would drop the -0.0 tokens.
 __device__ __forceinline__ uint32_t fkey(float f) {
-  const uint32_t u = __float_as_uint(f);
+  const uint32_t u = f == 0.f ? 0u : __float_as_uint(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
@@ -175,7 +179,8 @@ __device__ uint4 philox4x32_10(uint2 key, uint4 c) {
   return c;
 }
 
-__global__ void __launch_bounds__(kSampleThreads) sample_random_kernel(SampleArgs a) {
+// 4 CTAs per SM (32 registers): a 512-row chunk then runs in one wave on 132 SMs
+__global__ void __launch_bounds__(kSampleThreads, 4) sample_random_kernel(SampleArgs a) {
   const int b = blockIdx.x;
   const int slot = a.row_slot[b];
   if (a.slot_done[slot]) return;
@@ -191,10 +196,10 @@ __global__ void __launch_bounds__(kSampleThreads) sample_random_kernel(SampleArg
   __shared__ float sv[kSampleWarps];
   __shared__ int si[kSampleWarps];
   __shared__ uint32_t hist_u[256];
-  __shared__ float hist_f[256];
+  __shared__ unsigned long long hist_m[256];
   __shared__ uint32_t sh_prefix, sh_pmask;
   __shared__ int sh_k;
-  __shared__ float sh_above;
+  __shared__ unsigned long long sh_above, sh_target;
   __shared__ float wsum[kSampleWarps + 1];
   __shared__ int sh_tok;
 
@@ -204,7 +209,7 @@ __global__ void __launch_bounds__(kSampleThreads) sample_random_kernel(SampleArg
     if (allowed(i)) m = better(m, ArgMax{lg[i] * inv_t, i});
   m = block_argmax(m, sv, si);
   if (m.i < 0 || m.i >= V) {  // nothing selectable
-    if (threadIdx.x == 0) finish_row(a, slot, state, a.eos_id, 0.f);
+    if (threadIdx.x == 0) finish_row(a, slot, state, a.eos_id, 0.f, true);
     return;
   }
   const float zmax = m.v;
@@ -240,46 +245,65 @@ __global__ void __launch_bounds__(kSampleThreads) sample_random_kernel(SampleArg
       __syncthreads();
     }
     tau = sh_prefix;
+    __syncthreads();  // every thread holds tau before the top-p descent reuses sh_prefix
   }
 
-  // 3. softmax mass of the (top-k filtered) set; top-p threshold on the same ordering
-  float W = 0.f;
-  for (int i = threadIdx.x; i < V; i += kSampleThreads) {
-    if (!allowed(i)) continue;
-    const float z = lg[i] * inv_t;
-    if (fkey(z) >= tau) W += __expf(z - zmax);
-  }
-  W = block_sum(W, sv);
+  // 3. top-p threshold on the same ordering, weighted by the softmax mass exp(z - zmax) of the
+  //    (top-k filtered) set.  The masses are summed in 24.40 fixed point (the largest weight is
+  //    1, so V < 2^24 terms cannot overflow 64 bits): integer sums do not depend on the order of
+  //    the atomics, so the kept set is a function of the logits alone.  Rounding each weight to
+  //    2^-40 moves the mass of the whole row by less than V * 2^-41 <= 2e-7 (W >= 1).
   if (a.top_p < 1.0f) {
-    const float target = a.top_p * W;
-    if (threadIdx.x == 0) sh_prefix = 0, sh_pmask = 0, sh_above = 0.f;
+    if (threadIdx.x == 0) sh_prefix = 0, sh_pmask = 0, sh_above = 0ull;
     for (int shift = 24; shift >= 0; shift -= 8) {
-      for (int i = threadIdx.x; i < 256; i += kSampleThreads) hist_f[i] = 0.f;
+      for (int i = threadIdx.x; i < 256; i += kSampleThreads) hist_m[i] = 0ull;
       __syncthreads();
       const uint32_t prefix = sh_prefix, pmask = sh_pmask;
-      for (int i = threadIdx.x; i < V; i += kSampleThreads) {
-        if (!allowed(i)) continue;
-        const float z = lg[i] * inv_t;
-        const uint32_t key = fkey(z);
-        if (key >= tau && (key & pmask) == prefix)
-          atomicAdd(&hist_f[(key >> shift) & 255u], __expf(z - zmax));
+      const int lane = threadIdx.x & 31;
+      for (int base = threadIdx.x & ~31; base < V; base += kSampleThreads) {  // warp-uniform
+        const int i = base + lane;
+        uint32_t bin = 0u;
+        unsigned long long w = 0ull;
+        bool in = false;
+        if (i < V && allowed(i)) {
+          const float z = lg[i] * inv_t;
+          const uint32_t key = fkey(z);
+          in = key >= tau && (key & pmask) == prefix;
+          bin = (key >> shift) & 255u;
+          if (in) w = __float2ull_rn(__expf(z - zmax) * 1099511627776.0f);  // * 2^40
+        }
+        // one shared atomic per distinct bin of the warp; w <= 2^40 is summed as two 20-bit
+        // halves so that 32 lanes cannot overflow the 32-bit warp reduction
+        for (unsigned todo = __ballot_sync(~0u, in); todo != 0u;) {
+          const int lead = __ffs(todo) - 1;
+          const uint32_t b0 = __shfl_sync(~0u, bin, lead);
+          const bool mine = in && bin == b0;
+          todo &= ~__ballot_sync(~0u, mine);
+          const uint32_t lo = __reduce_add_sync(~0u, mine ? static_cast<uint32_t>(w) & 0xFFFFFu : 0u);
+          const uint32_t hi = __reduce_add_sync(~0u, mine ? static_cast<uint32_t>(w >> 20) : 0u);
+          if (lane == lead) atomicAdd(&hist_m[b0], (static_cast<unsigned long long>(hi) << 20) + lo);
+        }
       }
       __syncthreads();
       if (threadIdx.x == 0) {
-        float cum = sh_above;
-        int sel = -1, last = 0;
+        if (shift == 24) {  // the first pass sees the whole set: target = ceil(top_p * W)
+          unsigned long long w = 0ull;
+          for (int bin = 0; bin < 256; ++bin) w += hist_m[bin];
+          sh_target =
+              static_cast<unsigned long long>(ceil(fmax(0.0, static_cast<double>(a.top_p)) * w));
+        }
+        // The bin chosen by the previous pass holds exactly the mass of this pass's bins, so
+        // some non-empty bin reaches the target (top_p < 1 puts it at or below W).
+        const unsigned long long target = sh_target;
+        unsigned long long cum = sh_above;
+        int sel = 0;
         for (int bin = 255; bin >= 0; --bin) {
-          const float c = hist_f[bin];
-          if (c > 0.f) last = bin;
-          if (c > 0.f && cum + c >= target) {
+          const unsigned long long c = hist_m[bin];
+          if (c > 0ull && cum + c >= target) {
             sel = bin;
             break;
           }
           cum += c;
-        }
-        if (sel < 0) {  // rounding: the tail never quite reached the target -> keep everything
-          sel = last;
-          cum -= hist_f[last];
         }
         sh_above = cum;
         sh_prefix = prefix | (static_cast<uint32_t>(sel) << shift);
@@ -362,7 +386,10 @@ __global__ void __launch_bounds__(kSampleThreads) sample_random_kernel(SampleArg
     se = block_sum(se, sv);
     logprob = (lg[tok] * inv_t - zmax) - __logf(se);
   }
-  if (threadIdx.x == 0) finish_row(a, slot, state, tok, logprob);
+  if (threadIdx.x == 0) {
+    if (a.out_tau != nullptr) a.out_tau[b] = tau;
+    finish_row(a, slot, state, tok, logprob);
+  }
 }
 
 __global__ void prepare_decode_kernel(const int32_t* __restrict__ row_slot,

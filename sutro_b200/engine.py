@@ -112,6 +112,22 @@ class ResultC(C.Structure):          # sb200_result (include/sutro_b200.h)
                 ("embeddings", C.POINTER(C.c_float)), ("d_model", C.c_int)]
 
 
+class SampleArgsC(C.Structure):     # sb200_sample_args (test hook: one sampling step)
+    _fields_ = [("logits", C.c_void_p), ("ldl", C.c_int), ("vocab", C.c_int), ("B", C.c_int)] + \
+               [(n, C.c_void_p) for n in ("row_slot", "slot_state", "slot_ngen", "slot_next_tok",
+                                          "slot_pos", "slot_done", "slot_row", "slot_maxnew",
+                                          "out_tokens", "out_len")] + \
+               [("out_stride", C.c_int), ("mask_bits", C.c_void_p), ("mask_words", C.c_int)] + \
+               [(n, C.c_void_p) for n in ("fsm_trans", "fsm_accept", "fsm_final", "fsm_tail_off",
+                                          "fsm_tail_tok", "tok_bytes", "tok_off")] + \
+               [("eos_id", C.c_int), ("ignore_eos", C.c_int), ("temperature", C.c_float),
+                ("top_k", C.c_int), ("top_p", C.c_float), ("seed", C.c_uint64),
+                ("seed_per_row", C.c_int)] + \
+               [(n, C.c_void_p) for n in ("row_ids", "slot_cum_logprob", "out_cum_logprob",
+                                          "out_tau")]
+
+
+L.register("sb200_sample", C.c_int, [C.POINTER(SampleArgsC), C.c_void_p])
 L.register("sb200_engine_info", C.c_int, [C.c_void_p] + [C.POINTER(C.c_int)] * 4)
 L.register("sb200_infer_text", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                          C.POINTER(JobC), C.c_int, C.c_int,

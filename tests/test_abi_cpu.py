@@ -64,7 +64,8 @@ def test_ctypes_struct_layouts_match_the_header(tmp_path):
         pytest.skip("gcc not available")
     from sutro_b200 import engine as E
     mirrors = {"sb200_engine_config": E.EngineConfigC, "sb200_engine_weights": E.EngineWeightsC,
-               "sb200_job": E.JobC, "sb200_job_stats": E.JobStatsC, "sb200_result": E.ResultC}
+               "sb200_job": E.JobC, "sb200_job_stats": E.JobStatsC, "sb200_result": E.ResultC,
+               "sb200_sample_args": E.SampleArgsC}
     lines = ['#include <stdio.h>', '#include <stddef.h>', f'#include "{HEADER}"', "int main(void){"]
     for cname, mirror in mirrors.items():
         lines.append(f'printf("{cname} size %zu\\n", sizeof({cname}));')

@@ -74,3 +74,29 @@ def test_kept_sets_match_transformers_logits_warpers():
         assert (keep == theirs).all(), (trial, T, k, p, keep.sum(), theirs.sum())
         checked += 1
     assert checked > 40
+
+
+def test_vectorised_philox_matches_the_scalar_one():
+    f = 0xffffffff
+    for key, ctr in [((0, 0), (0, 0, 0, 0)), ((f, f), (f, f, f, f)),
+                     ((0xa4093822, 0x299f31d0), (0x243f6a88, 0x85a308d3, 0x13198a2e, 0x03707344))]:
+        assert tuple(int(x) for x in S.philox4x32_10_np(key, ctr)) == S.philox4x32_10(key, ctr)
+    rows = np.array([0, 5, 2 ** 32 + 7, 2 ** 63 - 1], dtype=np.uint64)
+    steps = np.array([0, 1, 2 ** 31 - 1, 12345])
+    for spr in (False, True):
+        u = np.broadcast_to(S.uniform_np(2 ** 40 + 3, rows, steps, spr), 4)
+        assert [float(x) for x in u] == [S.uniform(2 ** 40 + 3, int(r), int(s), spr)
+                                         for r, s in zip(rows, steps)]
+
+
+def test_fkey_order_and_exact_thresholds():
+    z = np.array([-np.inf, -3.0, -1e-40, -0.0, 0.0, 1e-40, 2.0, np.inf], dtype=np.float32)
+    k = S.fkey(z)
+    assert (np.diff(k.astype(np.int64)) >= 0).all() and k[3] == k[4]
+    lg = np.array([5, 4, 4, 4, 1], dtype=np.float32)
+    allowed = np.ones(5, dtype=bool)
+    assert S.tau_expected(lg, allowed, 1.0, 3, 1.0) == (S.fkey(np.float32(4)), np.inf)
+    assert S.tau_expected(lg, allowed, 1.0, 9, 1.0)[0] == 0                # k > allowed: off
+    tau, margin = S.tau_expected(lg, allowed, 1.0, 0, 0.5)                 # 1 / 2.12 < 0.5
+    assert tau == S.fkey(np.float32(4)) and abs(margin - (0.5 - 1 / 2.1219)) < 1e-3
+    assert S.scaled(np.float32(3.0), 0.7) == np.float32(3.0) * (np.float32(1) / np.float32(0.7))

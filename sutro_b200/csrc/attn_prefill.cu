@@ -79,11 +79,9 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __rest
     const uint32_t bar = smem_u32(&full_bar[stage]);
     const uint32_t dst = smem_u32(smem + stage * kPfStageBytes);
     mbar_arrive_expect_tx(bar, two ? 4 * kTileBytes : 2 * kTileBytes);
-    bulk_load_1d(dst, kv_layer + (static_cast<size_t>(s_pt[p0]) * hkv + kvh) * (2 * kTileElems),
-                 2 * kTileBytes, bar);
+    bulk_load_1d(dst, kv_layer + kv_tile_offset(s_pt[p0], hkv, kvh, true), 2 * kTileBytes, bar);
     if (two)
-      bulk_load_1d(dst + 2 * kTileBytes,
-                   kv_layer + (static_cast<size_t>(s_pt[p0 + 1]) * hkv + kvh) * (2 * kTileElems),
+      bulk_load_1d(dst + 2 * kTileBytes, kv_layer + kv_tile_offset(s_pt[p0 + 1], hkv, kvh, true),
                    2 * kTileBytes, bar);
   };
   if (threadIdx.x == 0) {
@@ -146,7 +144,7 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __rest
       for (int kk = 0; kk < 8; ++kk) {
         const int tok = (lm >> 1) * 8 + lr;
         const int chunk = kk * 2 + (lm & 1);
-        const uint32_t off = tok * 256 + ((chunk ^ (tok & 7)) << 4);
+        const uint32_t off = tok * 256 + (kv_chunk(tok, chunk) << 4);
         uint32_t b0, b1, b2, b3;
         ldmatrix_x4(base + off, b0, b1, b2, b3);
         mma_bf16_16816(s[0], qa[kk], b0, b1);
@@ -200,7 +198,7 @@ attn_prefill_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __rest
       for (int nt = 0; nt < 16; nt += 2) {
         const int tok = (lm & 1) * 8 + lr;
         const int chunk = nt + (lm >> 1);
-        const uint32_t off = kTileBytes + tok * 256 + ((chunk ^ (tok & 7)) << 4);
+        const uint32_t off = kTileBytes + tok * 256 + (kv_chunk(tok, chunk) << 4);
         o[nt][0] *= alpha[0];
         o[nt][1] *= alpha[0];
         o[nt][2] *= alpha[1];
@@ -265,28 +263,15 @@ int attn_prefill(const void* qkv, void* out, const void* kv_layer, const int32_t
                  const int32_t* seq_q_start, const int32_t* seq_q_len, const int32_t* seq_past,
                  int hq, int hkv, float scale, cudaStream_t stream) {
   if (n_work <= 0) return 0;
-  if (hkv <= 0 || hq % hkv != 0) {
-    set_last_error("attn_prefill: hq=%d not a multiple of hkv=%d", hq, hkv);
-    return -1;
-  }
   if (max_pages > kPfMaxPages) {
     set_last_error("attn_prefill: max_pages=%d exceeds the staged page-table size %d", max_pages,
                    kPfMaxPages);
     return -1;
   }
-#define SB_PF(G)                                                                               \
-  return launch<G>(qkv, out, kv_layer, page_table, max_pages, work, n_work, seq_slot,         \
-                   seq_q_start, seq_q_len, seq_past, hq, hkv, scale, stream)
-  switch (hq / hkv) {
-    case 1: SB_PF(1);
-    case 2: SB_PF(2);
-    case 4: SB_PF(4);
-    case 8: SB_PF(8);
-    default:
-      set_last_error("attn_prefill: unsupported GQA group size %d", hq / hkv);
-      return -1;
-  }
-#undef SB_PF
+  return dispatch_gqa("attn_prefill", hq, hkv, [&](auto g) {
+    return launch<g.value>(qkv, out, kv_layer, page_table, max_pages, work, n_work, seq_slot,
+                           seq_q_start, seq_q_len, seq_past, hq, hkv, scale, stream);
+  });
 }
 
 }  // namespace sb

@@ -408,29 +408,16 @@ int attn_prefill_dense(const void* qkv, int t_rows, void* out, const void* prefi
                        const int32_t* seq_past, int hq, int hkv, float scale,
                        cudaStream_t stream) {
   if (n_items <= 0) return 0;
-  if (hkv <= 0 || hq % hkv != 0) {
-    set_last_error("attn_prefill_dense: hq=%d not a multiple of hkv=%d", hq, hkv);
-    return -1;
-  }
   if (layer < 0 || layer >= std::max(n_layers, 1)) {
     set_last_error("attn_prefill_dense: layer %d out of range", layer);
     return -1;
   }
-  TcMaps m;
-  if (tc_maps(TcKey{qkv, prefix_kv, t_rows, hq, hkv, prefix_rows, n_layers}, &m)) return -1;
-#define SB_TC(G)                                                                             \
-  return launch_tc<G>(m, out, items, n_items, seq_q_start, seq_q_len, seq_past, hq, hkv,    \
-                      prefix_kv ? layer : 0, scale, stream)
-  switch (hq / hkv) {
-    case 1: SB_TC(1);
-    case 2: SB_TC(2);
-    case 4: SB_TC(4);
-    case 8: SB_TC(8);
-    default:
-      set_last_error("attn_prefill_dense: unsupported GQA group size %d", hq / hkv);
-      return -1;
-  }
-#undef SB_TC
+  return dispatch_gqa("attn_prefill_dense", hq, hkv, [&](auto g) {
+    TcMaps m;
+    if (tc_maps(TcKey{qkv, prefix_kv, t_rows, hq, hkv, prefix_rows, n_layers}, &m)) return -1;
+    return launch_tc<g.value>(m, out, items, n_items, seq_q_start, seq_q_len, seq_past, hq, hkv,
+                              prefix_kv ? layer : 0, scale, stream);
+  });
 }
 
 }  // namespace sb

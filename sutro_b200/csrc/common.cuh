@@ -10,6 +10,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace sb {
 
 #define SB_DEVICE __device__ __forceinline__
@@ -29,6 +31,26 @@ void set_last_error(const char* fmt, ...);
       return -1;                                                                    \
     }                                                                               \
   } while (0)
+
+// GQA group dispatch of the attention launchers: checks that hq is a multiple of hkv and calls
+// f(std::integral_constant<int, G>{}) for G = hq / hkv, one of the group sizes the kernels are
+// instantiated for.  Errors are reported as "<who>: ..." and return -1.
+template <class F>
+int dispatch_gqa(const char* who, int hq, int hkv, F&& f) {
+  if (hkv <= 0 || hq % hkv != 0) {
+    set_last_error("%s: hq=%d not a multiple of hkv=%d", who, hq, hkv);
+    return -1;
+  }
+  switch (hq / hkv) {
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 2: return f(std::integral_constant<int, 2>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 8: return f(std::integral_constant<int, 8>{});
+    default:
+      set_last_error("%s: unsupported GQA group size %d", who, hq / hkv);
+      return -1;
+  }
+}
 
 // cudaFuncSetAttribute is per device: remember, per call site, on which devices the
 // dynamic-shared-memory limit has already been raised (one engine per GPU may live in the

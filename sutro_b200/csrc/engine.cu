@@ -254,7 +254,7 @@ struct Engine {
     logit_rows = std::min(std::max(c.logit_chunk_rows, 1), std::max(c.max_slots, 1));
     q_tile = attn_prefill_q_tile(c.n_q_heads, c.n_kv_heads);
     num_pages = c.num_pages;
-    layer_stride = static_cast<size_t>(num_pages) * c.n_kv_heads * 2 * kTileElems;
+    layer_stride = num_pages * kv_page_elems(c.n_kv_heads);
     if (const char* e = getenv("SB200_FUSE_QKV")) fuse_qkv = e[0] != '0';
     if (const char* e = getenv("SB200_PREFILL_TC")) prefill_tc = e[0] != '0';
     SB_CUDA_CHECK(cudaGetDevice(&device));
@@ -608,7 +608,7 @@ int Engine::run(const sb200_job& job, sb200_job_stats* stats) {
     if (prefix_tail_page >= 0 && sample) {
       ++prof.launches[SB200_KC_OTHER];
       copy_prefix_page_kernel<<<dim3(n, c.n_layers), 256, 0, stream>>>(
-          kv_pool, layer_stride, static_cast<size_t>(c.n_kv_heads) * 2 * kTileElems,
+          kv_pool, layer_stride, kv_page_elems(c.n_kv_heads),
           prefix_tail_page, d_copy);
     }
     SB_CUDA_CHECK(cudaGetLastError());

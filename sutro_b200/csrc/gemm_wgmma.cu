@@ -175,8 +175,7 @@ SB_DEVICE void qkv_row_meta(const QkvEpiArgs& ea, int row, bool row_ok, QkvRowMe
   if (row_ok) {
     rm.pos = ea.tok_pos[row];
     const int slot = ea.tok_slot[row];
-    rm.page = static_cast<size_t>(
-        ea.page_table[static_cast<size_t>(slot) * ea.max_pages + rm.pos / kPageTokens]);
+    rm.page = static_cast<size_t>(kv_page(ea.page_table, ea.max_pages, slot, rm.pos));
     rm.r = rm.pos % kPageTokens;
   }
 }
@@ -229,15 +228,16 @@ SB_DEVICE void qkv_head_epilogue(const float (&acc)[R], int hh, const QkvEpiArgs
     const float rstd = nw != nullptr ? rsqrtf(ss / static_cast<float>(kHeadDim) + ea.eps) : 1.f;
     __nv_bfloat16* dst_lo;
     __nv_bfloat16* dense = qkv_out + static_cast<size_t>(row) * ldd + head * kHeadDim;
+    // chunk c of the row is stored at c ^ swz: kv_chunk(r, c) == c ^ kv_chunk(r, 0), taken out of
+    // the loop below (q heads are not swizzled)
     int swz = 0;
     if (is_q) {
       dst_lo = dense;
     } else {
       const int kvh = is_k ? (head - ea.hq) : (head - ea.hq - ea.hkv);
       dst_lo = static_cast<__nv_bfloat16*>(ea.kv_layer) +
-               (rm[h].page * ea.hkv + kvh) * (2 * kTileElems) + (is_k ? 0 : kTileElems) +
-               rm[h].r * kHeadDim;
-      swz = rm[h].r & 7;
+               kv_tile_offset(rm[h].page, ea.hkv, kvh, is_k) + rm[h].r * kHeadDim;
+      swz = kv_chunk(rm[h].r, 0);
     }
     const __nv_bfloat16* cosr =
         static_cast<const __nv_bfloat16*>(ea.cos_tab) + static_cast<size_t>(rm[h].pos) * 64;

@@ -24,6 +24,24 @@ constexpr int kPageTokens = 16;
 constexpr int kTileElems = kPageTokens * kHeadDim;   // one K (or V) tile of one head
 constexpr int kTileBytes = kTileElems * 2;           // 4096
 
+// The layout above in code: every kernel that reads or writes the pool, and every host-side
+// size of it, goes through these.
+// elements of one page of one layer: the K and V tiles of every kv head
+__host__ __device__ inline size_t kv_page_elems(int hkv) {
+  return static_cast<size_t>(hkv) * 2 * kTileElems;
+}
+// element offset, within one layer, of the K (is_k) or V tile of kv head kvh of a page; the
+// V tile directly follows the K tile, so one copy of 2 * kTileBytes from the K tile fetches both
+__host__ __device__ inline size_t kv_tile_offset(size_t page, int hkv, int kvh, bool is_k) {
+  return (page * hkv + kvh) * (2 * kTileElems) + (is_k ? 0 : kTileElems);
+}
+// stored position of the 16-byte chunk c of token row r of a tile
+__host__ __device__ inline int kv_chunk(int r, int c) { return c ^ (r & 7); }
+// physical page that holds position pos of the sequence in slot `slot` (row pos % kPageTokens)
+__host__ __device__ inline int kv_page(const int32_t* page_table, int max_pages, int slot, int pos) {
+  return page_table[static_cast<size_t>(slot) * max_pages + pos / kPageTokens];
+}
+
 enum GemmEpilogue {
   EPI_STORE_BF16 = 0,
   EPI_RESIDUAL_BF16 = 1,

@@ -316,7 +316,7 @@ int sb200_model_open(const char* dir, int device, int max_slots, int max_prefill
     if (kv_pages <= 0) {  // 80 % of what is free after the weights, capped at every slot full
       size_t free_b = 0, total_b = 0;
       SB_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-      const int64_t page_bytes = 2LL * c.n_layers * c.n_kv_heads * kHeadDim * 2 * kPageTokens;
+      const int64_t page_bytes = 2LL * c.n_layers * kv_page_elems(c.n_kv_heads);  // all layers, bf16
       const int64_t t_max = std::max(c.max_prefill_tokens, c.max_slots);
       const int64_t act = t_max * 2LL * (2LL * c.d_model + (c.n_q_heads + 2LL * c.n_kv_heads) * kHeadDim +
                                          c.n_q_heads * kHeadDim + c.d_ff) +

@@ -131,7 +131,7 @@ rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __restrict_
   const int l = threadIdx.x & 15;
   const int pos = tok_pos[t];
   const int slot = tok_slot[t];
-  const int page = page_table[static_cast<size_t>(slot) * max_pages + pos / kPageTokens];
+  const int page = kv_page(page_table, max_pages, slot, pos);
   const int r = pos % kPageTokens;
   const int nheads = hq + 2 * hkv;
   __nv_bfloat16* row = qkv + static_cast<size_t>(t) * nheads * kHeadDim;
@@ -203,14 +203,12 @@ rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __restrict_
       *reinterpret_cast<uint2*>(hp + 64 + 4 * l) = phi;
     } else {
       const int kvh = is_k ? (hh - hq) : (hh - hq - hkv);
-      __nv_bfloat16* tile = kv_layer +
-                            (static_cast<size_t>(page) * hkv + kvh) * (2 * kTileElems) +
-                            (is_k ? 0 : kTileElems) + r * kHeadDim;
+      __nv_bfloat16* tile = kv_layer + kv_tile_offset(page, hkv, kvh, is_k) + r * kHeadDim;
       const int c_lo = l >> 1;             // 16-byte chunk holding dims 4l..4l+3
       const int c_hi = c_lo + 8;
       const int within = (4 * l) & 7;      // 0 or 4 elements into the chunk
-      *reinterpret_cast<uint2*>(tile + ((c_lo ^ (r & 7)) << 3) + within) = plo;
-      *reinterpret_cast<uint2*>(tile + ((c_hi ^ (r & 7)) << 3) + within) = phi;
+      *reinterpret_cast<uint2*>(tile + (kv_chunk(r, c_lo) << 3) + within) = plo;
+      *reinterpret_cast<uint2*>(tile + (kv_chunk(r, c_hi) << 3) + within) = phi;
       if (is_k) {  // dense copy for the wgmma prefill attention (V is already in place)
         *reinterpret_cast<uint2*>(hp + 4 * l) = plo;
         *reinterpret_cast<uint2*>(hp + 64 + 4 * l) = phi;

@@ -46,6 +46,30 @@ def test_python_binding_table_matches_header():
     _lib.lib()
 
 
+@pytest.mark.skipif(not os.path.exists(LIB), reason="library not built")
+@pytest.mark.parametrize("hq,hkv,msg", [
+    (12, 4, "unsupported GQA group size 3"),
+    (12, 0, "hq=12 not a multiple of hkv=0"),
+])
+def test_attention_launchers_reject_unsupported_gqa_groups(hq, hkv, msg):
+    """The GQA group is checked before any CUDA call, so this needs no GPU."""
+    lib = ctypes.CDLL(LIB)
+    lib.sb200_last_error.restype = ctypes.c_char_p
+    ints = (ctypes.c_int32 * 4)()
+    scale = ctypes.c_float(1.0)
+    calls = {
+        "attn_decode": lambda: lib.sb200_attn_decode(
+            None, None, None, ints, 1, ints, ints, 1, hq, hkv, scale, None),
+        "attn_prefill": lambda: lib.sb200_attn_prefill(
+            None, None, None, ints, 1, ints, 1, ints, ints, ints, ints, hq, hkv, scale, None),
+        "attn_prefill_dense": lambda: lib.sb200_attn_prefill_dense(
+            None, 1, None, None, 0, 1, 0, ints, 1, ints, ints, ints, hq, hkv, scale, None),
+    }
+    for who, call in calls.items():
+        assert call() == -1, who
+        assert lib.sb200_last_error().decode() == f"{who}: {msg}"
+
+
 def test_no_product_module_imports_the_oracle():
     pkg = os.path.join(ROOT, "sutro_b200")
     for dirpath, _, files in os.walk(pkg):

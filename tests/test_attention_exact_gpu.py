@@ -28,6 +28,7 @@ import pytest
 import torch
 
 from sutro_b200 import _lib as L
+import bf16_ref as R
 import kv_layout as KV
 
 DEV = "cuda"
@@ -850,19 +851,6 @@ def rope_tables(max_pos=4096, theta=1e6):
     return bf(fr.cos()).to(DEV), bf(fr.sin()).to(DEV)
 
 
-def rmsnorm_ref(x, w, eps=1e-6):
-    xf = x.float()
-    return bf(w.float() * bf(xf * torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + eps)).float())
-
-
-def rope_ref(x, cos, sin):
-    """x: [T, H, 128] bf16, cos/sin: [T, 64] — rotate-half RoPE, every op rounded to bf16."""
-    c = torch.cat([cos, cos], -1)[:, None, :]
-    s = torch.cat([sin, sin], -1)[:, None, :]
-    rot = torch.cat([-x[..., 64:], x[..., :64]], -1)
-    return (x * c) + (rot * s)
-
-
 def fused_qkv(a, m, w, qn, kn, cos, sin, tok_slot, tok_pos, pt, pool, hq, hkv, block_n, out):
     d_slot, d_pos, d_pt = i32(tok_slot), i32(tok_pos), i32(pt)
     L.check(L.lib().sb200_gemm_qkv_rope(
@@ -872,9 +860,6 @@ def fused_qkv(a, m, w, qn, kn, cos, sin, tok_slot, tok_pos, pt, pool, hq, hkv, b
     torch.cuda.synchronize()
 
 
-QK_DIFF_LIMIT = 0.005   # fraction of q/k elements that may differ from the op-by-op oracle
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("M", [77, 129, 300])
 @pytest.mark.parametrize("qk_norm", [True, False], ids=["qk_norm", "no_norm"])
@@ -882,10 +867,11 @@ QK_DIFF_LIMIT = 0.005   # fraction of q/k elements that may differ from the op-b
 def test_qkv_epilogue_dense_kv_copy(block_n, qk_norm, M):
     """Small-integer A and W make the projection exact.  The k/v columns of the output must be
     bit-identical to what the same launch wrote into the pool, V must be bf16(A Wv^T), Q and K
-    must match linear -> bf16 -> RMSNorm -> RoPE (bit for bit without the norm; within one bf16
-    ulp at the RoPE operands' scale, on at most QK_DIFF_LIMIT of the elements, with it: the
-    kernel's rsqrtf and sum order differ from torch's), at positions up to 4095.  Output rows
-    >= M and pool slots no token maps to stay untouched."""
+    must match linear -> bf16 -> RMSNorm -> RoPE bit for bit, at positions up to 4095; with the
+    norm, an output whose normed operand (dim i or i + 64) is tied may take either rounding of it
+    (bf16_ref: the epilogue rounds x * rstd to bf16 and then uses exact bf16x2 products, so the
+    window of the fp32 sum of squares and rsqrtf is all that matters).  Output rows >= M and pool
+    slots no token maps to stay untouched."""
     hq, hkv, K, extra = 32, 8, 256, 40
     N = (hq + 2 * hkv) * HD
     torch.manual_seed(M + block_n + int(qk_norm))
@@ -921,17 +907,13 @@ def test_qkv_epilogue_dense_kv_copy(block_n, qk_norm, M):
 
     pos = tok_pos.to(DEV)
     for name, sl, nw in (("q", slice(0, hq), qn), ("k", slice(hq, hq + hkv), kn)):
-        x = rmsnorm_ref(lin[:, sl], nw) if qk_norm else lin[:, sl]
-        ref = rope_ref(x, cos[pos], sin[pos])
-        g = got[:, sl]
-        if not qk_norm:
-            assert torch.equal(g, ref), name
-            continue
-        opnd = torch.maximum(x[..., :64].abs(), x[..., 64:].abs()).float().repeat(1, 1, 2)
-        scale = torch.maximum(ref.float().abs(), opnd)
-        diff = (g.float() - ref.float()).abs()
-        assert torch.all(diff <= ulp_bf16(scale)), (name, (diff / ulp_bf16(scale)).max().item())
-        assert (diff > 0).float().mean().item() <= QK_DIFF_LIMIT, name
+        cands, tied = R.normed_rope_candidates(lin[:, sl], nw, 1e-6, R.QKV_NORM_DEPTH, cos[pos],
+                                               sin[pos])
+        R.assert_one_of(got[:, sl], cands, name)
+        if qk_norm:
+            print(f"[ties] fused QKV {name} M={M} block_n={block_n}: "
+                  f"{tied.double().mean().item():.2e} tied")
+            assert tied.double().mean().item() < 0.01, name
 
 
 @pytest.mark.gpu

@@ -11,6 +11,8 @@ import torch
 from sutro_b200 import _lib as L
 import kv_layout as KV
 from test_attention_exact_gpu import assert_within_bound, attn_ref64
+from test_gemm_epilogue_gpu import (RESIDUAL_BF16, STORE_BF16, SWIGLU_BF16,
+                                    assert_f32_within_bound, check_against_f32, interleave, tiles)
 
 pytestmark = pytest.mark.gpu
 
@@ -47,15 +49,12 @@ def _gemm(a, w, epi=0, resid=None, block_n=0, m=None, out=None):
 @pytest.mark.parametrize("M,N,K", [(128, 256, 64), (128, 256, 256), (300, 768, 512),
                                    (1000, 1536, 2560), (77, 32 * 11, 192)])
 def test_gemm_store_bf16(M, N, K, block_n):
+    """bf16(acc) bit for bit, and the accumulator within the fp64 bound."""
     torch.manual_seed(M * 7 + N + K)
     a = bf(torch.randn(M, K, device=DEV))
     w = bf(torch.randn(N, K, device=DEV) / math.sqrt(K))
-    d = _gemm(a, w, 0, block_n=block_n)
-    ref = a.float() @ w.float().t()
-    err = (d.float() - ref).abs().max().item()
-    assert err <= 2e-2 * max(1.0, ref.abs().max().item()), err
-    # bf16 rounding of the exact fp32 result: at most 1 bf16 ulp away
-    assert torch.allclose(d.float(), bf(ref).float(), rtol=1.6e-2, atol=1e-3)
+    acc = check_against_f32(a, w, STORE_BF16, M, block_n)
+    assert_f32_within_bound(acc, a, w, f"store_bf16 {M}x{N}x{K} block_n={block_n}")
 
 
 def test_gemm_exact_integers():
@@ -101,17 +100,13 @@ def test_gemm_exact_integers_at_the_benchmark_shapes(M, N, K, epi):
 
 
 def test_gemm_swiglu_at_the_benchmark_shape():
+    """SwiGLU at a full prefill step of qwen-3-4b, bit for bit under the SiLU tie rule against
+    the fp32 accumulator of the same launch shape."""
     M, F, K = 16384, 9728, 2560
     torch.manual_seed(11)
     a = bf(torch.randn(M, K, device=DEV))
     w = bf(torch.randn(2 * F, K, device=DEV) / math.sqrt(K))
-    d = _gemm(a, w, 2)
-    acc = a.float() @ w.float().t()
-    g, u = bf(acc[:, 0::2]).float(), bf(acc[:, 1::2]).float()
-    ref = bf(bf(torch.nn.functional.silu(g)).float() * u)
-    assert d.shape == (M, F)
-    assert torch.allclose(d.float(), ref.float(), rtol=3e-2, atol=2e-2)
-    assert (d != ref).float().mean().item() < 0.02       # rounding-boundary cases only
+    check_against_f32(a, w, SWIGLU_BF16, M)
 
 
 def test_gemm_tile_configurations_are_bit_identical():
@@ -152,17 +147,8 @@ def test_gemm_cta_pair_fused_epilogues(epi):
     torch.manual_seed(7)
     a = bf(torch.randn(M, K, device=DEV))
     w = bf(torch.randn(N, K, device=DEV) / math.sqrt(K))
-    acc = a.float() @ w.float().t()
-    if epi == 1:
-        r = bf(torch.randn(M, N, device=DEV))
-        out = r.clone()
-        _gemm(a, w, 1, resid=out, out=out, block_n=512)
-        ref = bf(bf(acc).float() + r.float())
-    else:
-        out = _gemm(a, w, 2, block_n=512)
-        g, u = bf(acc[:, 0::2]).float(), bf(acc[:, 1::2]).float()
-        ref = bf(bf(torch.nn.functional.silu(g)).float() * u)
-    assert torch.allclose(out.float(), ref.float(), rtol=3e-2, atol=3e-2)
+    r = bf(torch.randn(tiles(M), N, device=DEV))
+    check_against_f32(a, w, epi, M, block_n=512, resid=r if epi == RESIDUAL_BF16 else None)
 
 
 def test_gemm_residual():
@@ -170,11 +156,8 @@ def test_gemm_residual():
     torch.manual_seed(3)
     a = bf(torch.randn(M, K, device=DEV))
     w = bf(torch.randn(N, K, device=DEV) / math.sqrt(K))
-    r = bf(torch.randn(M, N, device=DEV))
-    out = r.clone()
-    _gemm(a, w, 1, resid=out, out=out)  # in place, as the engine does
-    ref = bf(bf(a.float() @ w.float().t()).float() + r.float())
-    assert torch.allclose(out.float(), ref.float(), rtol=1.6e-2, atol=2e-2)
+    r = bf(torch.randn(tiles(M), N, device=DEV))
+    check_against_f32(a, w, RESIDUAL_BF16, M, resid=r)  # in place, as the engine does
 
 
 def test_gemm_swiglu():
@@ -183,13 +166,10 @@ def test_gemm_swiglu():
     a = bf(torch.randn(M, K, device=DEV))
     wg = bf(torch.randn(F, K, device=DEV) / math.sqrt(K))
     wu = bf(torch.randn(F, K, device=DEV) / math.sqrt(K))
-    w = torch.stack([wg, wu], dim=1).reshape(2 * F, K).contiguous()  # interleaved rows
-    d = _gemm(a, w, 2)
-    g = bf(a.float() @ wg.float().t()).float()
-    u = bf(a.float() @ wu.float().t()).float()
-    ref = bf(bf(torch.nn.functional.silu(g)).float() * u)
-    assert d.shape == (M, F)
-    assert torch.allclose(d.float(), ref.float(), rtol=3e-2, atol=2e-2)
+    acc = check_against_f32(a, interleave(wg, wu), SWIGLU_BF16, M)
+    # the accumulator's even columns are the gate projection, the odd ones the up projection
+    assert_f32_within_bound(acc[:, 0::2], a, wg, "swiglu gate")
+    assert_f32_within_bound(acc[:, 1::2], a, wu, "swiglu up")
 
 
 def test_gemm_f32_logits_partial_n_tile():
@@ -198,9 +178,7 @@ def test_gemm_f32_logits_partial_n_tile():
     a = bf(torch.randn(M, K, device=DEV))
     w = bf(torch.randn(N, K, device=DEV) / math.sqrt(K))
     for bn in (64, 128, 256, 512):
-        d = _gemm(a, w, 3, block_n=bn)
-        ref = a.float() @ w.float().t()
-        assert torch.allclose(d, ref, rtol=1e-3, atol=1e-3), bn
+        assert_f32_within_bound(_gemm(a, w, 3, block_n=bn), a, w, f"logits block_n={bn}")
 
 
 def test_gemm_bad_shape_reports_error():
@@ -213,26 +191,6 @@ def test_gemm_bad_shape_reports_error():
 
 
 # --------------------------------------------------------------------------- row kernels
-def rmsnorm_ref(x, w, eps):
-    xf = x.float()
-    var = xf.pow(2).mean(-1, keepdim=True)
-    return bf(w.float() * bf(xf * torch.rsqrt(var + eps)).float())
-
-
-@pytest.mark.parametrize("rows,d", [(1, 128), (37, 1024), (513, 2560)])
-def test_rmsnorm(rows, d):
-    torch.manual_seed(rows)
-    x = bf(torch.randn(rows, d, device=DEV) * 3)
-    w = bf(torch.randn(d, device=DEV))
-    out = torch.empty_like(x)
-    L.check(L.lib().sb200_rmsnorm(L.ptr(x), L.ptr(w), L.ptr(out), rows, d, 1e-6, stream()))
-    torch.cuda.synchronize()
-    ref = rmsnorm_ref(x, w, 1e-6)
-    # rsqrtf vs torch.rsqrt may differ by an ulp -> allow one bf16 step on a few elements
-    assert torch.allclose(out.float(), ref.float(), rtol=1e-2, atol=1e-2)
-    assert (out != ref).float().mean().item() < 0.02
-
-
 def test_embed_gather_and_l2norm():
     torch.manual_seed(0)
     table = bf(torch.randn(1000, 256, device=DEV))
@@ -248,67 +206,11 @@ def test_embed_gather_and_l2norm():
     assert torch.allclose(o32, ref, rtol=1e-5, atol=1e-6)
 
 
+# --------------------------------------------------------------------------- fused QKV
 def rope_tables(max_pos, theta=1e6):
     inv = 1.0 / (theta ** (torch.arange(0, KV.HD, 2, dtype=torch.float32) / KV.HD))
     fr = torch.arange(max_pos, dtype=torch.float32)[:, None] * inv[None, :]
     return bf(fr.cos()).to(DEV), bf(fr.sin()).to(DEV)
-
-
-def rope_ref(x, cos, sin):
-    """x: [T, H, 128] bf16; cos/sin: [T, 64] bf16 — bf16 op-by-op like transformers."""
-    c = torch.cat([cos, cos], -1)[:, None, :]
-    s = torch.cat([sin, sin], -1)[:, None, :]
-    x1, x2 = x[..., :64], x[..., 64:]
-    rot = torch.cat([-x2, x1], -1)
-    return (x * c) + (rot * s)  # bf16 tensors: each op rounds to bf16
-
-
-@pytest.mark.parametrize("qk_norm", [True, False])
-def test_rope_kv_write(qk_norm):
-    torch.manual_seed(11)
-    hq, hkv, T = 8, 2, 50
-    n_slots, max_pages, num_pages = 3, 8, 40
-    qkv = bf(torch.randn(T, (hq + 2 * hkv) * KV.HD, device=DEV))
-    qn = bf(torch.rand(KV.HD, device=DEV) + 0.5) if qk_norm else None
-    kn = bf(torch.rand(KV.HD, device=DEV) + 0.5) if qk_norm else None
-    cos, sin = rope_tables(256)
-    tok_slot = torch.randint(0, n_slots, (T,), dtype=torch.int32)
-    # unique (slot, pos) pairs
-    tok_pos = torch.zeros(T, dtype=torch.int32)
-    seen = {}
-    for t in range(T):
-        s = int(tok_slot[t])
-        seen[s] = seen.get(s, 3)  # start at position 3 -> exercises non-zero offsets
-        tok_pos[t] = seen[s]
-        seen[s] += 1
-    pt = torch.randperm(num_pages)[: n_slots * max_pages].view(n_slots, max_pages).to(torch.int32)
-    pool = torch.zeros(num_pages, hkv, 2, KV.PAGE, KV.HD, dtype=torch.bfloat16, device=DEV)
-    orig = qkv.clone()
-    # keep device copies alive across the launch (temporaries would be recycled)
-    d_slot, d_pos, d_pt = tok_slot.to(DEV), tok_pos.to(DEV), pt.to(DEV)
-    L.check(L.lib().sb200_rope_kv_write(
-        L.ptr(qkv), L.ptr(qn), L.ptr(kn), L.ptr(cos), L.ptr(sin), L.ptr(d_slot),
-        L.ptr(d_pos), L.ptr(d_pt), max_pages, L.ptr(pool), T, hq, hkv, 1e-6,
-        stream()))
-    torch.cuda.synchronize()
-    x = orig.view(T, hq + 2 * hkv, KV.HD)
-    q, k, v = x[:, :hq], x[:, hq:hq + hkv], x[:, hq + hkv:]
-    if qk_norm:
-        q = rmsnorm_ref(q, qn, 1e-6)
-        k = rmsnorm_ref(k, kn, 1e-6)
-    pos = tok_pos.long().to(DEV)
-    q_ref = rope_ref(q, cos[pos], sin[pos])
-    k_ref = rope_ref(k, cos[pos], sin[pos])
-    got_q = qkv.view(T, hq + 2 * hkv, KV.HD)[:, :hq]
-    assert torch.allclose(got_q.float(), q_ref.float(), rtol=2e-2, atol=2e-2)
-    assert (got_q != q_ref).float().mean().item() < 0.02
-    logical = KV.unpack_tile(pool)  # [pages, hkv, 2, 16, 128]
-    for t in range(T):
-        page = int(pt[int(tok_slot[t]), int(tok_pos[t]) // KV.PAGE])
-        r = int(tok_pos[t]) % KV.PAGE
-        assert torch.allclose(logical[page, :, 0, r].float(), k_ref[t].float(), rtol=2e-2,
-                              atol=2e-2)
-        assert torch.equal(logical[page, :, 1, r], v[t])
 
 
 @pytest.mark.parametrize("block_n", [128, 256, 512, 0])

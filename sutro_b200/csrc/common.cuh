@@ -225,6 +225,40 @@ SB_DEVICE void tma_load_3d(uint32_t smem_dst, const CUtensorMap* m, uint32_t bar
       "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// 2-D tiled store shared -> global into the issuing thread's current bulk group; the parts of
+// the box outside the tensor map's dims are not written.
+SB_DEVICE void tma_store_2d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_src), "r"(c0), "r"(c1)
+               : "memory");
+}
+SB_DEVICE void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// Wait until at most N of this thread's bulk groups still read their shared-memory source.
+template <int N>
+SB_DEVICE void bulk_wait_group_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// Wait until at most N of this thread's bulk groups are incomplete (their writes done).
+template <int N>
+SB_DEVICE void bulk_wait_group() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+// Barrier `id` (1..15; 0 is __syncthreads) over the first `count` threads to arrive.
+SB_DEVICE void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+SB_DEVICE void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+SB_DEVICE void st_shared_b16(uint32_t addr, uint16_t v) {
+  asm volatile("st.shared.b16 [%0], %1;" ::"r"(addr), "h"(v) : "memory");
+}
+SB_DEVICE uint32_t ld_shared_b32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
 // 1-D bulk copy global -> shared (no tensor map; size multiple of 16 B).
 SB_DEVICE void bulk_load_1d(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
   asm volatile(

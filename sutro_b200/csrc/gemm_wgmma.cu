@@ -9,20 +9,27 @@
 //   warps 0-7  two consumer warpgroups: warpgroup c owns rows [64c, 64c+64) of the 128-row
 //              tile and issues wgmma.m64nBLOCK_Nk16 (four per 64-element K block) straight
 //              from the shared-memory ring, accumulating in registers; one K block stays in
-//              flight while the next is issued.  The fused epilogue runs from the registers.
+//              flight while the next is issued.  The fused epilogue rounds the registers into
+//              the warpgroup's 64-row slab of a staging buffer, and one thread stores the slab
+//              with TMA; the warpgroup goes on to the next tile's mainloop while it drains.
 //   warps 8-11 producer warpgroup (gives its registers to the consumers); warp 8 issues the
 //              cp.async.bulk.tensor 2-D loads of A (128x64) and W (BLOCK_N x 64) tiles into a
 //              kStages-deep ring and runs ahead into the next tile while the consumers are in
-//              their epilogue.
+//              their epilogue.  For RESIDUAL_BF16, warp 9 loads each slab's residual tile into
+//              the staging buffer by TMA as soon as the slab's previous store has read it out,
+//              so the load overlaps the tile's mainloop.
 //
 // Fused epilogues (rounding points mirror the bf16 oracle, oracle/model_ref.py):
 //   STORE_BF16     D = bf16(acc)
 //   RESIDUAL_BF16  D = bf16(bf16(acc) + R)           (O-proj / down-proj + residual)
 //   SWIGLU_BF16    D[:, j] = bf16(silu(bf16(acc[2j])) * bf16(acc[2j+1]))
 //                  (gate/up weights interleaved row-wise; output has N/2 columns)
-//   STORE_F32      D = acc                             (lm_head logits)
+//   STORE_F32      D = acc                             (lm_head logits; stored from the registers:
+//                  its 128 x 256 fp32 tile does not fit beside the ring)
 //   QKV_ROPE       q/k RMSNorm + RoPE, K/V into the paged cache and into their columns of D
 //                  (the dense copy the prefill attention reads; see qkv_head_epilogue)
+// TMA clips every store and residual load at the tensor map's dims (M rows, N or N/2 columns),
+// so rows >= M and columns past N are never written.
 #include <algorithm>
 #include <cstdlib>
 #include <mutex>
@@ -47,11 +54,36 @@ struct GemmCfg {
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  // ~192 KiB of ring for every tile width (the limit is 227 KiB per block)
-  static constexpr int kStages = (BLOCK_N == 256) ? 4 : (BLOCK_N == 128 ? 6 : 8);
+  // The limit is 227 KiB per block: ~192 KiB of ring beside the staging buffer for the 64- and
+  // 128-wide tiles; the 256-wide tile gives up its fourth stage to stage the whole tile.
+  static constexpr int kStages = (BLOCK_N == 256) ? 3 : (BLOCK_N == 128 ? 6 : 8);
+  static constexpr int kSlabBytes = 64 * BLOCK_N * 2;   // one warpgroup's 64 rows, bf16
   static constexpr int kBarBytes = 256;
-  static constexpr int kSmemBytes = kStages * kStageBytes + kBarBytes + 1024;  // +align slack
+  static constexpr int kSmemBytes =
+      kStages * kStageBytes + 2 * kSlabBytes + kBarBytes + 1024;   // +align slack
+  static_assert(kSmemBytes <= 232448, "shared memory per block");
 };
+
+// The bf16 output of one tile: kCols columns (N/2 per tile for SwiGLU), staged and stored as
+// boxes of 64 rows x kBoxCols columns.
+template <int BLOCK_N, int EPI>
+struct EpiCfg {
+  static constexpr int kCols = EPI == EPI_SWIGLU_BF16 ? BLOCK_N / 2 : BLOCK_N;
+  static constexpr int kBoxCols = kCols < 64 ? kCols : 64;
+  static constexpr int kBoxes = kCols / kBoxCols;
+  static constexpr int kBoxBytes = 64 * kBoxCols * 2;
+};
+
+// Byte offset of (row r, column c) in a staging slab: boxes of 64 rows x BOX_COLS columns back
+// to back, each in the TMA swizzle of its row width (128-byte rows: SWIZZLE_128B, 64-byte rows:
+// SWIZZLE_64B).  The swizzle also puts the 16 bytes a quad writes in each of eight consecutive
+// rows into different banks.
+template <int BOX_COLS>
+SB_DEVICE uint32_t stage_off(int r, int c) {
+  const uint32_t off = r * (BOX_COLS * 2) + (c % BOX_COLS) * 2;
+  return (c / BOX_COLS) * (64 * BOX_COLS * 2) +
+         (off ^ (((off >> 7) & (BOX_COLS == 64 ? 7 : 3)) << 4));
+}
 
 template <int BN>
 SB_DEVICE void wgmma_ss(float (&d)[BN / 2], uint64_t adesc, uint64_t bdesc) {
@@ -73,85 +105,53 @@ SB_DEVICE void tile_to_mn(int GM, int tile, int num_m, int num_n, int& m_blk, in
   n_blk = within / gm;
 }
 
-// This thread's accumulators (rows row0 and row0 + 8, columns col0 + 8j + {0, 1}) -> fused
-// epilogue -> global.  col0 already includes the lane's 2 * (lane % 4).
-// RESIDUAL_BF16: D = bf16(bf16(acc) + R), R read from HBM.  Loaded one element pair before
-// its store, as the compiler schedules a plain loop, only a few loads are in flight per thread
-// and the epilogue becomes a chain of memory round trips that kept the tensor cores idle for
-// longer than the mainloop of a K = 4096 tile (O-projection at 0.35 of the rate of the same
-// GEMM with a plain bf16 store).  So the loads of a chunk of kChunk column groups are issued
-// together, then the chunk is rounded, summed and stored: four round trips per 256-wide tile.
-// A chunk of 16 spills: ptxas allots 168 registers, 128 of them accumulators.
-template <int BLOCK_N>
-SB_DEVICE void epilogue_residual(const float (&acc)[BLOCK_N / 2], __nv_bfloat16* d_out,
-                                 const __nv_bfloat16* resid, int row0, int col0, int M, int N,
-                                 int ldd) {
-  constexpr int kChunk = 8;
+// The thread's accumulators: acc[4j + 2h + e] is row 8h of the thread's rows, column
+// 8j + 2 * (lane % 4) + e of the tile.
+
+// STORE_BF16, SWIGLU_BF16, RESIDUAL_BF16 -> the warpgroup's staging slab; srow is the slab row
+// of the thread's first row, q = lane % 4.  For RESIDUAL_BF16 the slab already holds R (loaded
+// by TMA), which is read and overwritten in place: D = bf16(bf16(acc) + R).
+template <int BLOCK_N, int EPI>
+SB_DEVICE void epilogue_stage(const float (&acc)[BLOCK_N / 2], uint32_t slab, int srow, int q) {
+  using Epi = EpiCfg<BLOCK_N, EPI>;
 #pragma unroll
-  for (int j0 = 0; j0 < BLOCK_N / 8; j0 += kChunk) {
-    uint32_t r[kChunk][2];
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
 #pragma unroll
-    for (int j = 0; j < kChunk; ++j) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int col = col0 + 8 * (j0 + j), row = row0 + 8 * h;
-        // volatile: the compiler would otherwise sink each load to its use again
-        asm volatile(
-            "{\n.reg .pred p;\nsetp.ne.b32 p, %2, 0;\nmov.b32 %0, 0;\n"
-            "@p ld.global.b32 %0, [%1];\n}\n"
-            : "=r"(r[j][h])
-            : "l"(resid + static_cast<size_t>(row) * ldd + col), "r"(int(col < N && row < M)));
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < kChunk; ++j) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int col = col0 + 8 * (j0 + j), row = row0 + 8 * h;
-        if (col < N && row < M) {
-          const float2 rv = unpack_bf16x2(r[j][h]);
-          const int i = 4 * (j0 + j) + 2 * h;
-          *reinterpret_cast<uint32_t*>(d_out + static_cast<size_t>(row) * ldd + col) =
-              pack_bf16x2(bf16_round(acc[i]) + rv.x, bf16_round(acc[i + 1]) + rv.y);
+    for (int h = 0; h < 2; ++h) {
+      const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      if constexpr (EPI == EPI_SWIGLU_BF16) {
+        // gate/up columns 2c, 2c + 1 give output column c = 4j + q
+        const float g = bf16_round(v0);
+        const float u = bf16_round(v1);
+        const float s = bf16_round(g / (1.0f + __expf(-g)));
+        st_shared_b16(slab + stage_off<Epi::kBoxCols>(srow + 8 * h, 4 * j + q),
+                      __bfloat16_as_ushort(__float2bfloat16_rn(s * u)));
+      } else {
+        const uint32_t a = slab + stage_off<64>(srow + 8 * h, 8 * j + 2 * q);
+        if constexpr (EPI == EPI_RESIDUAL_BF16) {
+          const float2 rv = unpack_bf16x2(ld_shared_b32(a));
+          st_shared_b32(a, pack_bf16x2(bf16_round(v0) + rv.x, bf16_round(v1) + rv.y));
+        } else {
+          st_shared_b32(a, pack_bf16x2(v0, v1));
         }
       }
     }
   }
 }
 
-// STORE_BF16, SWIGLU_BF16, STORE_F32.
-template <int BLOCK_N, int EPI>
-SB_DEVICE void epilogue_store(const float (&acc)[BLOCK_N / 2], void* __restrict__ d_out,
-                              int row0, int col0, int M, int N, int ldd) {
-  const int lane = threadIdx.x & 31;
+// STORE_F32 (rows row0 and row0 + 8, columns col0 + 8j + {0, 1}; col0 includes 2 * (lane % 4)).
+template <int BLOCK_N>
+SB_DEVICE void epilogue_store_f32(const float (&acc)[BLOCK_N / 2], float* __restrict__ d_out,
+                                  int row0, int col0, int M, int N, int ldd) {
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int col = col0 + 8 * j;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = row0 + 8 * h;
-      const bool ok = col < N && row < M;
-      const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-      const size_t off = static_cast<size_t>(row) * ldd + col;
-      if constexpr (EPI == EPI_SWIGLU_BF16) {
-        const float g = bf16_round(v0);
-        const float u = bf16_round(v1);
-        const float s = bf16_round(g / (1.0f + __expf(-g)));
-        // output column col/2: the even lane of a pair stores its own and its neighbour's
-        const uint32_t mine = __bfloat16_as_ushort(__float2bfloat16_rn(s * u));
-        const uint32_t other = __shfl_xor_sync(0xffffffffu, mine, 1);
-        if (ok && (lane & 1) == 0)
-          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(d_out) +
-                                       static_cast<size_t>(row) * ldd + (col >> 1)) =
-              mine | (other << 16);
-      } else if (ok) {
-        if constexpr (EPI == EPI_STORE_F32) {
-          *reinterpret_cast<float2*>(reinterpret_cast<float*>(d_out) + off) = make_float2(v0, v1);
-        } else {
-          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(d_out) + off) =
-              pack_bf16x2(v0, v1);
-        }
-      }
+      if (col < N && row < M)
+        *reinterpret_cast<float2*>(d_out + static_cast<size_t>(row) * ldd + col) =
+            make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
     }
   }
 }
@@ -159,9 +159,10 @@ SB_DEVICE void epilogue_store(const float (&acc)[BLOCK_N / 2], void* __restrict_
 // ---------------------------------------------------------------------------
 // EPI_QKV_ROPE: per 128-column head, each row gets exactly what rope_kv_kernel (norm_rope.cu)
 // does to the stored bf16 tensor — bf16 rounding of the projection, optional per-head RMSNorm,
-// rotate-half RoPE with bf16 op-by-op rounding — then q heads go to the qkv buffer and k/v
-// heads straight into the swizzled KV page (and, unswizzled, into their columns of the qkv
-// buffer for the dense prefill attention).  A row's head is spread over the four lanes of a
+// rotate-half RoPE with bf16 op-by-op rounding — then every head goes to the staging slab (q
+// heads for the qkv buffer; k/v heads for their columns of it, the dense copy the prefill
+// attention reads, stored only with write_dense) and k/v heads straight from the registers into
+// the swizzled KV page as well (the page of each row is its own).  A row's head is spread over the four lanes of a
 // quad (32 dims each); dim d and its RoPE partner d + 64 sit in the same thread, so only the
 // sum of squares needs two shuffles.
 // ---------------------------------------------------------------------------
@@ -183,7 +184,7 @@ SB_DEVICE void qkv_row_meta(const QkvEpiArgs& ea, int row, bool row_ok, QkvRowMe
 template <int R>
 SB_DEVICE void qkv_head_epilogue(const float (&acc)[R], int hh, const QkvEpiArgs& ea,
                                  const QkvRowMeta (&rm)[2], int row0, int M, int head, bool head_ok,
-                                 __nv_bfloat16* __restrict__ qkv_out, int ldd) {
+                                 uint32_t slab, int srow) {
   const int q = threadIdx.x & 3;
   const bool is_q = head < ea.hq;
   const bool is_k = !is_q && head < ea.hq + ea.hkv;
@@ -226,17 +227,14 @@ SB_DEVICE void qkv_head_epilogue(const float (&acc)[R], int hh, const QkvEpiArgs
     ss += __shfl_xor_sync(0xffffffffu, ss, 2);
     if (!head_ok || row >= M) continue;
     const float rstd = nw != nullptr ? rsqrtf(ss / static_cast<float>(kHeadDim) + ea.eps) : 1.f;
-    __nv_bfloat16* dst_lo;
-    __nv_bfloat16* dense = qkv_out + static_cast<size_t>(row) * ldd + head * kHeadDim;
-    // chunk c of the row is stored at c ^ swz: kv_chunk(r, c) == c ^ kv_chunk(r, 0), taken out of
-    // the loop below (q heads are not swizzled)
+    // K/V page row; chunk c of the row is stored at c ^ swz: kv_chunk(r, c) == c ^ kv_chunk(r, 0),
+    // taken out of the loop below
+    __nv_bfloat16* kv_lo = nullptr;
     int swz = 0;
-    if (is_q) {
-      dst_lo = dense;
-    } else {
+    if (!is_q) {
       const int kvh = is_k ? (head - ea.hq) : (head - ea.hq - ea.hkv);
-      dst_lo = static_cast<__nv_bfloat16*>(ea.kv_layer) +
-               kv_tile_offset(rm[h].page, ea.hkv, kvh, is_k) + rm[h].r * kHeadDim;
+      kv_lo = static_cast<__nv_bfloat16*>(ea.kv_layer) +
+              kv_tile_offset(rm[h].page, ea.hkv, kvh, is_k) + rm[h].r * kHeadDim;
       swz = kv_chunk(rm[h].r, 0);
     }
     const __nv_bfloat16* cosr =
@@ -261,13 +259,13 @@ SB_DEVICE void qkv_head_epilogue(const float (&acc)[R], int hh, const QkvEpiArgs
         lo = sub2(mul2(x, c), mul2(y, s));
         hi = add2(mul2(y, c), mul2(x, s));
       }
-      *reinterpret_cast<uint32_t*>(dst_lo + ((jj ^ swz) << 3) + 2 * q) = lo;
-      *reinterpret_cast<uint32_t*>(dst_lo + (((jj + 8) ^ swz) << 3) + 2 * q) = hi;
-      if (!is_q && ea.write_dense) {
-        // dense copy next to q: the dense prefill attention reads the new tokens' K/V from the
-        // qkv buffer through TMA (attn_prefill_tc.cu); decode reads the paged copy above
-        *reinterpret_cast<uint32_t*>(dense + d) = lo;
-        *reinterpret_cast<uint32_t*>(dense + 64 + d) = hi;
+      st_shared_b32(slab + stage_off<64>(srow + 8 * h, 128 * hh + d), lo);
+      st_shared_b32(slab + stage_off<64>(srow + 8 * h, 128 * hh + 64 + d), hi);
+      if (!is_q) {
+        // the dense prefill attention reads the new tokens' K/V from the qkv buffer through TMA
+        // (attn_prefill_tc.cu); decode reads this paged copy
+        *reinterpret_cast<uint32_t*>(kv_lo + ((jj ^ swz) << 3) + 2 * q) = lo;
+        *reinterpret_cast<uint32_t*>(kv_lo + (((jj + 8) ^ swz) << 3) + 2 * q) = hi;
       }
     }
   }
@@ -276,17 +274,24 @@ SB_DEVICE void qkv_head_epilogue(const float (&acc)[R], int hh, const QkvEpiArgs
 template <int BLOCK_N, int EPI>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
-                    const __grid_constant__ CUtensorMap tm_b, void* __restrict__ d_out,
-                    const __nv_bfloat16* __restrict__ resid, int M, int N, int K, int ldd,
-                    int ea_gm, const QkvEpiArgs ea) {
+                    const __grid_constant__ CUtensorMap tm_b,
+                    const __grid_constant__ CUtensorMap tm_d,   // bf16 output (not STORE_F32)
+                    const __grid_constant__ CUtensorMap tm_r,   // residual (RESIDUAL_BF16)
+                    float* __restrict__ d_f32, int M, int N, int K, int ldd, int ea_gm,
+                    const QkvEpiArgs ea) {
   using Cfg = GemmCfg<BLOCK_N>;
+  using Epi = EpiCfg<BLOCK_N, EPI>;
+  constexpr bool kStaged = EPI != EPI_STORE_F32;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint8_t* staging = smem + Cfg::kStages * Cfg::kStageBytes;   // two warpgroup slabs
+  uint64_t* bars = reinterpret_cast<uint64_t*>(staging + 2 * Cfg::kSlabBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + Cfg::kStages;
+  uint64_t* slab_free = bars + 2 * Cfg::kStages;   // per slab: its last store has read it out
+  uint64_t* resid_full = slab_free + 2;            // per slab: the tile's residual has landed
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -294,9 +299,15 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
   if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&tm_a);
     tma_prefetch_desc(&tm_b);
+    if constexpr (kStaged) tma_prefetch_desc(&tm_d);
+    if constexpr (EPI == EPI_RESIDUAL_BF16) tma_prefetch_desc(&tm_r);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
       mbar_init(smem_u32(&empty_bar[s]), kConsumerWarps);
+    }
+    for (int c = 0; c < 2; ++c) {
+      mbar_init(smem_u32(&slab_free[c]), 1);
+      mbar_init(smem_u32(&resid_full[c]), 1);
     }
     fence_mbar_init();
   }
@@ -329,6 +340,26 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
           }
         }
       }
+    } else if (EPI == EPI_RESIDUAL_BF16 && warp == kProducerWarp + 1 && lane == 0) {
+      // residual loader: R of each slab, as soon as the slab's previous store has read it out.
+      // In place (R == D, as the engine runs it) is safe: tiles are disjoint, and a tile's R is
+      // loaded before its D is stored.  Boxes wholly past M or N are not loaded.
+      uint32_t it = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+        int m_blk, n_blk;
+        tile_to_mn(ea_gm, tile, num_m, num_n, m_blk, n_blk);
+        for (int c = 0; c < 2; ++c) {
+          const int row = m_blk * kBlockM + 64 * c;
+          const uint32_t bar = smem_u32(&resid_full[c]);
+          const uint32_t dst = smem_u32(staging + c * Cfg::kSlabBytes);
+          int boxes = 0;
+          if (row < M) boxes = min(Epi::kBoxes, (N - n_blk * BLOCK_N + 63) / 64);
+          mbar_wait_long(smem_u32(&slab_free[c]), (it & 1) ^ 1);
+          mbar_arrive_expect_tx(bar, boxes * Epi::kBoxBytes);
+          for (int b = 0; b < boxes; ++b)
+            tma_load_2d(dst + b * Epi::kBoxBytes, &tm_r, bar, n_blk * BLOCK_N + 64 * b, row);
+        }
+      }
     }
     return;
   }
@@ -337,12 +368,17 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
   setmaxnreg_inc<232>();
   const int wg = warp >> 2;   // rows [64 wg, 64 wg + 64) of the tile
   const uint32_t smem0 = smem_u32(smem);
+  const uint32_t slab = smem_u32(staging + wg * Cfg::kSlabBytes);
+  const int srow = (warp & 3) * 16 + (lane >> 2);   // slab row of the thread's first row
+  // issues the warpgroup's TMA stores, and waits for them (bulk groups belong to one thread)
+  const bool leader = (threadIdx.x & 127) == 0;
   int stage = 0;
   uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+  uint32_t it = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
     int m_blk, n_blk;
     tile_to_mn(ea_gm, tile, num_m, num_n, m_blk, n_blk);
-    const int row0 = m_blk * kBlockM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int row0 = m_blk * kBlockM + wg * 64 + srow;
     QkvRowMeta rm[2];
     if constexpr (EPI == EPI_QKV_ROPE) {   // overlaps the mainloop's loads
       qkv_row_meta(ea, row0, row0 < M, rm[0]);
@@ -361,6 +397,14 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
       for (int k = 0; k < kBlockK / 16; ++k)
         wgmma_ss<BLOCK_N>(acc, gmma_desc_k_sw128(sa + 32 * k), gmma_desc_k_sw128(sb + 32 * k));
       wgmma_commit();
+      if constexpr (EPI == EPI_RESIDUAL_BF16) {
+        // with the first K block issued, hand the slab to the residual loader once the previous
+        // tile's store has read it out
+        if (kb == 0 && it > 0 && leader) {
+          bulk_wait_group_read<0>();
+          mbar_arrive(smem_u32(&slab_free[wg]));
+        }
+      }
       // the previous K block has retired once at most this one is in flight: free its stage
       wgmma_wait<1>();
       if (prev >= 0) {
@@ -379,23 +423,43 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
       __syncwarp();
       if (lane == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
     }
+    if constexpr (EPI == EPI_STORE_F32) {
+      epilogue_store_f32<BLOCK_N>(acc, d_f32, row0, n_blk * BLOCK_N + 2 * (lane & 3), M, N, ldd);
+      continue;
+    }
+    if constexpr (EPI == EPI_RESIDUAL_BF16) {
+      mbar_wait(smem_u32(&resid_full[wg]), it & 1);
+    } else {
+      // the slab's previous store has had this tile's mainloop to read it out
+      if (leader) bulk_wait_group_read<0>();
+      named_bar_sync(1 + wg, 128);
+    }
     if constexpr (EPI == EPI_QKV_ROPE) {
       static_assert(BLOCK_N % 128 == 0 || EPI != EPI_QKV_ROPE, "fused QKV needs whole heads");
 #pragma unroll
       for (int hh = 0; hh < BLOCK_N / 128; ++hh) {
         const int head = (n_blk * BLOCK_N) / kHeadDim + hh;
-        qkv_head_epilogue(acc, hh, ea, rm, row0, M, head, head * kHeadDim < N,
-                          reinterpret_cast<__nv_bfloat16*>(d_out), ldd);
+        qkv_head_epilogue(acc, hh, ea, rm, row0, M, head, head * kHeadDim < N, slab, srow);
       }
-    } else if constexpr (EPI == EPI_RESIDUAL_BF16) {
-      // in place (resid == d_out) in the engine: each element is read before it is written,
-      // by the same thread
-      epilogue_residual<BLOCK_N>(acc, reinterpret_cast<__nv_bfloat16*>(d_out), resid, row0,
-                                 n_blk * BLOCK_N + 2 * (lane & 3), M, N, ldd);
     } else {
-      epilogue_store<BLOCK_N, EPI>(acc, d_out, row0, n_blk * BLOCK_N + 2 * (lane & 3), M, N, ldd);
+      epilogue_stage<BLOCK_N, EPI>(acc, slab, srow, lane & 3);
+    }
+    fence_proxy_async_smem();   // this thread's slab writes, before the async proxy reads them
+    named_bar_sync(1 + wg, 128);
+    if (leader) {
+      const int row = m_blk * kBlockM + 64 * wg;
+      const int n_out = EPI == EPI_SWIGLU_BF16 ? N / 2 : N;
+      for (int b = 0; b < Epi::kBoxes; ++b) {
+        const int col = n_blk * Epi::kCols + b * Epi::kBoxCols;
+        // decode (write_dense = 0) leaves the K/V columns of the qkv buffer untouched
+        const bool want = EPI != EPI_QKV_ROPE || ea.write_dense || col / kHeadDim < ea.hq;
+        if (row < M && col < n_out && want) tma_store_2d(&tm_d, slab + b * Epi::kBoxBytes, col, row);
+      }
+      bulk_commit_group();
     }
   }
+  // the stores must finish reading shared memory before the block exits
+  if (kStaged && leader) bulk_wait_group<0>();
 }
 
 // ---------------------------------------------------------------------------
@@ -468,6 +532,36 @@ int make_tmap(const void* ptr, int rows, int cols, int box_rows, CUtensorMap* ou
   }
   std::lock_guard<std::mutex> g(mu);
   cache.emplace(key, *out);
+  return 0;
+}
+
+// The bf16 output or residual of a fused epilogue: [rows, cols] with a row stride of ld
+// elements, box = 64 rows x box_cols columns in the swizzle of the staging slab (stage_off).
+// Encoded per launch, since M changes from call to call.
+int make_epi_tmap(const void* ptr, int rows, int cols, int ld, int box_cols, CUtensorMap* out) {
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (static_cast<long>(ld) * 2) % 16 != 0) {
+    set_last_error("gemm_bf16_tn: the bf16 output and residual need 16-byte aligned rows "
+                   "(ptr=%p ldd=%d)", ptr, ld);
+    return -1;
+  }
+  EncodeTiledFn enc = get_encode_fn();
+  if (!enc) {
+    set_last_error("cuTensorMapEncodeTiled entry point unavailable");
+    return -1;
+  }
+  cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * 2};
+  cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), 64};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides,
+                   box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_last_error("cuTensorMapEncodeTiled failed: %d (epilogue ptr=%p rows=%d cols=%d ldd=%d)",
+                   static_cast<int>(r), ptr, rows, cols, ld);
+    return -1;
+  }
   return 0;
 }
 
@@ -553,15 +647,21 @@ template <int BLOCK_N, int EPI>
 int launch_cfg(const void* a, int a_rows, const void* w, void* d, const void* resid, int M, int N,
                int K, int ldd, cudaStream_t stream, const QkvEpiArgs& ea) {
   using Cfg = GemmCfg<BLOCK_N>;
-  CUtensorMap tm_a, tm_b;
+  CUtensorMap tm_a, tm_b, tm_d{}, tm_r{};
   if (make_tmap(a, a_rows, K, kBlockM, &tm_a)) return -1;
   if (make_tmap(w, N, K, BLOCK_N, &tm_b)) return -1;
+  if constexpr (EPI != EPI_STORE_F32) {
+    using Epi = EpiCfg<BLOCK_N, EPI>;
+    if (make_epi_tmap(d, M, EPI == EPI_SWIGLU_BF16 ? N / 2 : N, ldd, Epi::kBoxCols, &tm_d))
+      return -1;
+    if (EPI == EPI_RESIDUAL_BF16 && make_epi_tmap(resid, M, N, ldd, 64, &tm_r)) return -1;
+  }
   auto kern = gemm_bf16_tn_kernel<BLOCK_N, EPI>;
   SB_SET_MAX_SMEM(kern, Cfg::kSmemBytes);
   const int tiles = ((M + kBlockM - 1) / kBlockM) * ((N + BLOCK_N - 1) / BLOCK_N);
   const int grid = tiles < num_sms() ? tiles : num_sms();
   kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(
-      tm_a, tm_b, d, reinterpret_cast<const __nv_bfloat16*>(resid), M, N, K, ldd,
+      tm_a, tm_b, tm_d, tm_r, reinterpret_cast<float*>(d), M, N, K, ldd,
       raster_group(kBlockM, N, K), ea);
   SB_CUDA_CHECK(cudaGetLastError());
   return 0;
@@ -616,7 +716,7 @@ int gemm_bf16_tn(const void* a, int a_rows, const void* w, void* d, const void* 
                  const QkvEpiArgs* qkv_args) {
   if (M <= 0) return 0;
   const QkvEpiArgs ea = qkv_args ? *qkv_args : QkvEpiArgs{};
-  if (K % kBlockK != 0 || N % 32 != 0 || a_rows < M) {
+  if (K <= 0 || K % kBlockK != 0 || N % 32 != 0 || a_rows < M) {
     set_last_error("gemm_bf16_tn: unsupported shape M=%d N=%d K=%d a_rows=%d", M, N, K, a_rows);
     return -1;
   }

@@ -1,6 +1,6 @@
 """Kernel-level timing of the bf16 GEMM at the qwen-3-4b prefill shapes (M = 32,768 tokens).
 
-    python tools/gemm_bench.py [--lib PATH] [--m ROWS] [--sweep] [--cublas] [--out FILE]
+    python tools/gemm_bench.py [--lib PATH] [--m ROWS] [--plain] [--sweep] [--cublas] [--out FILE]
 
 Times sb200_gemm_bf16_tn / sb200_gemm_qkv_rope with their real epilogues on seeded operands,
 with CUDA events over >= --seconds of work per shape after a warm-up, and prints one JSON line.
@@ -8,6 +8,8 @@ with CUDA events over >= --seconds of work per shape after a warm-up, and prints
               timed alternately on the same card
   --m         rows (tokens) per GEMM; the default is a full 32k-token prefill step, 128 or the
               decode batch (3584) time the decode-sized calls
+  --plain     also time each shape with a plain bf16 store (EPI_STORE_BF16 at the same N and K),
+              so the cost of each fused epilogue over a plain store can be read off directly
   --sweep     also time the down shape at block_n = 64 / 128 / 256 and report the implied
               operand feed, rate x (128 + BN) / (128 BN) bytes per flop into shared memory
   --cublas    also time torch.matmul (cuBLAS) at the same shapes and name its kernels
@@ -44,6 +46,7 @@ def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", default=None)
     ap.add_argument("--m", type=int, default=32768)
+    ap.add_argument("--plain", action="store_true")
     ap.add_argument("--sweep", action="store_true")
     ap.add_argument("--cublas", action="store_true")
     ap.add_argument("--seconds", type=float, default=1.0)
@@ -132,6 +135,14 @@ def main() -> None:
         del t["clock_sm"]
         res["shapes"][name] = {"N": N, "K": K, "epi": epi, **t}
         torch.cuda.empty_cache()
+
+    if args.plain:
+        res["plain"] = {}
+        for name, N, K, _ in SHAPES:
+            t = time_fn(make_call(N, K, 0, 0), 2.0 * M * N * K)
+            del t["clock_sm"]
+            res["plain"][name] = t
+            torch.cuda.empty_cache()
 
     if args.sweep:
         _, N, K, epi = SHAPES[1]

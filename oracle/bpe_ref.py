@@ -25,8 +25,10 @@ class RefTokenizer:
         self.v = v
         self.pat = regex.compile(PRETOK_PATTERN % v.digits)
         self.rank: Dict[Tuple[int, int], Tuple[int, int]] = {}
+        # a pair listed twice ranks at its last occurrence, as in `tokenizers` (its merge map is
+        # filled in list order, later entries replacing earlier ones)
         for i, (a, b) in enumerate(v.merges):
-            self.rank.setdefault((a, b), (i, 256 + i if v.merged_ids is None else v.merged_ids[i]))
+            self.rank[(a, b)] = (i, 256 + i if v.merged_ids is None else v.merged_ids[i])
         # ignore_merges: whole pre-token -> id, over the model vocabulary (not the added tokens)
         self.whole: Dict[bytes, int] = {}
         if v.word_overrides is not None:

@@ -15,8 +15,9 @@
 //      build something else): the host lists, for every such entry, the sequence its merges DO
 //      build; a pre-token whose merge result equals one of those sequences is replaced by the
 //      entry's id (two byte strings never merge to the same tokens, so the match is exact).
-//   3. exclusive scan (CUB) of the counts + compaction into the output.
-// HBM traffic: text bytes in, 4 B per token out, plus scratch at 4 B per byte.
+//   3. exclusive scan (CUB, 64-bit counts) of the counts + compaction into the output.
+// HBM traffic: text bytes in, 4 B per token out, plus scratch at 21 B per byte (flag, symbol,
+// count, output position).
 #include <cub/device/device_scan.cuh>
 
 #include <vector>
@@ -113,6 +114,12 @@ pretok_kernel(TokTables tb, const uint8_t* __restrict__ text, const int64_t* __r
       const uint8_t c1 = lower_ascii(p[1]);
       if (c1 == 's' || c1 == 't' || c1 == 'm' || c1 == 'd') {
         p += 2;
+        continue;
+      }
+      // U+017F LATIN SMALL LETTER LONG S (C5 BF) case-folds onto 's', so the pattern's (?i:'s)
+      // matches "'ſ"; it is the only non-ASCII code point that folds onto a contraction letter
+      if (p[1] == 0xC5 && p + 2 < end && p[2] == 0xBF) {
+        p += 3;
         continue;
       }
       if (p + 2 < end) {
@@ -217,7 +224,7 @@ __device__ __forceinline__ bool merge_lookup(const TokTables& tb, uint32_t a, ui
 
 __global__ void __launch_bounds__(256)
 bpe_kernel(TokTables tb, const uint8_t* __restrict__ text, int64_t n_bytes,
-           const uint8_t* __restrict__ flags, int32_t* __restrict__ sym, int32_t* __restrict__ cnt) {
+           const uint8_t* __restrict__ flags, int32_t* __restrict__ sym, int64_t* __restrict__ cnt) {
   const int64_t pos = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (pos >= n_bytes || !flags[pos]) return;
   int64_t e = pos + 1;
@@ -264,11 +271,11 @@ bpe_kernel(TokTables tb, const uint8_t* __restrict__ text, int64_t n_bytes,
 }
 
 __global__ void __launch_bounds__(256)
-compact_kernel(int64_t n_bytes, const int32_t* __restrict__ sym, const int32_t* __restrict__ cnt,
+compact_kernel(int64_t n_bytes, const int32_t* __restrict__ sym, const int64_t* __restrict__ cnt,
                const int64_t* __restrict__ outpos, int32_t* __restrict__ out_tokens) {
   const int64_t pos = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (pos >= n_bytes) return;
-  const int n = cnt[pos];
+  const int n = static_cast<int>(cnt[pos]);
   if (n == 0) return;
   int32_t* dst = out_tokens + outpos[pos];
   for (int i = 0; i < n; ++i) dst[i] = sym[pos + i];
@@ -285,7 +292,7 @@ __global__ void row_offsets_kernel(const int64_t* __restrict__ row_off, int64_t 
 // ---- detokeniser: token ids -> bytes --------------------------------------
 __global__ void __launch_bounds__(256)
 detok_len_kernel(const int32_t* __restrict__ toks, int64_t n, const int32_t* __restrict__ tok_off,
-                 int32_t* __restrict__ lens) {
+                 int64_t* __restrict__ lens) {
   const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (i > n) return;
   lens[i] = (i < n) ? (tok_off[toks[i] + 1] - tok_off[toks[i]]) : 0;
@@ -332,7 +339,9 @@ struct Tokenizer {
   int64_t cap = 0;
   uint8_t* d_flags = nullptr;
   int32_t* d_sym = nullptr;
-  int32_t* d_cnt = nullptr;
+  // per-position counts (tokens, or bytes when decoding) are 64-bit so that CUB's scan, which
+  // accumulates in its input type, does not wrap past 2^31 tokens or output bytes in one call
+  int64_t* d_cnt = nullptr;
   int64_t* d_outpos = nullptr;
   void* d_cub = nullptr;
   size_t cub_bytes = 0;
@@ -365,7 +374,7 @@ struct Tokenizer {
     cap = n + 1 + n / 4;
     SB_CUDA_CHECK(cudaMalloc(&d_flags, cap));
     SB_CUDA_CHECK(cudaMalloc(&d_sym, cap * sizeof(int32_t)));
-    SB_CUDA_CHECK(cudaMalloc(&d_cnt, cap * sizeof(int32_t)));
+    SB_CUDA_CHECK(cudaMalloc(&d_cnt, cap * sizeof(int64_t)));
     SB_CUDA_CHECK(cudaMalloc(&d_outpos, cap * sizeof(int64_t)));
     cub_bytes = 0;
     SB_CUDA_CHECK(cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, d_cnt, d_outpos, cap));
@@ -388,15 +397,9 @@ int tokenizer_create(const int32_t* merges, int n_merges, const int32_t* merged_
     const uint32_t a = merges[2 * i], b = merges[2 * i + 1];
     const uint64_t key = (static_cast<uint64_t>(a) << 32) | b;
     uint32_t h = pair_hash(a, b) & t->hmask;
-    bool dup = false;
-    while (keys[h] != kEmptyKey) {
-      if (keys[h] == key) {  // keep the first (lowest-rank) occurrence
-        dup = true;
-        break;
-      }
-      h = (h + 1) & t->hmask;
-    }
-    if (dup) continue;
+    while (keys[h] != kEmptyKey && keys[h] != key) h = (h + 1) & t->hmask;
+    // a pair listed twice takes the rank of its LAST occurrence: `tokenizers` builds its merge
+    // map by inserting the list in order, so a later entry replaces an earlier one
     keys[h] = key;
     const uint32_t id = merged_ids ? static_cast<uint32_t>(merged_ids[i]) : 256u + i;
     vals[h] = (static_cast<uint64_t>(i) << 32) | id;
@@ -487,7 +490,7 @@ int tokenizer_encode(Tokenizer* t, const uint8_t* text_dev, int64_t n_bytes,
                t->d_fkeys,  t->d_fslots, t->d_farena, t->fmask};
   const int64_t n1 = n_bytes + 1;
   SB_CUDA_CHECK(cudaMemsetAsync(t->d_flags, 0, n1, stream));
-  SB_CUDA_CHECK(cudaMemsetAsync(t->d_cnt, 0, n1 * sizeof(int32_t), stream));
+  SB_CUDA_CHECK(cudaMemsetAsync(t->d_cnt, 0, n1 * sizeof(int64_t), stream));
   if (n_bytes > 0) {
     pretok_kernel<<<static_cast<unsigned>((n_rows + 127) / 128), 128, 0, stream>>>(
         tb, text_dev, row_off_dev, n_rows, t->d_flags);

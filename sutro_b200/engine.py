@@ -228,11 +228,33 @@ def rows_to_blob(rows) -> Tuple[np.ndarray, np.ndarray]:
 
 
 def _nfc_rows(rows):
+    """NFC-normalised rows.  Arrow input stays Arrow: an all-ASCII column is already NFC and is
+    returned as is, any other is normalised row by row (`pyarrow.compute.utf8_normalize` is not
+    used: pyarrow 24.0 returns decomposed text for form "NFC").  Lists, pandas Series and other
+    iterables become lists with every string normalised (None and non-strings kept as they are,
+    rows_to_blob converts them)."""
     import unicodedata
-    if not isinstance(rows, (list, tuple)):
-        return rows            # Arrow / pandas input: taken as is
-    return [r if r is None or not isinstance(r, str) or unicodedata.is_normalized("NFC", r)
-            else unicodedata.normalize("NFC", r) for r in rows]
+
+    import pyarrow as pa
+
+    def nfc(rs):
+        return [r if r is None or not isinstance(r, str) or unicodedata.is_normalized("NFC", r)
+                else unicodedata.normalize("NFC", r) for r in rs]
+    if isinstance(rows, (pa.Array, pa.ChunkedArray)):
+        data, _ = rows_to_blob(rows)
+        if not (data >= 0x80).any():
+            return rows
+        return pa.array(nfc(rows.cast(pa.large_string()).to_pylist()), type=pa.large_string())
+    return nfc(rows)
+
+
+def normalize_rows(rows, vocab: Optional[VB.Vocab]):
+    """The rows as the vocabulary's tokenizer file wants them before pre-tokenisation: NFC when
+    it declares an NFC normalizer (Vocab.normalize_nfc, real Qwen files), unchanged otherwise.
+    Every entry point that tokenises host rows calls this, whatever the input form."""
+    if vocab is None or not vocab.normalize_nfc:
+        return rows
+    return _nfc_rows(rows)
 
 
 def _all_str(rows) -> bool:
@@ -655,8 +677,7 @@ class LocalEngine:
         emb_mode = self.spec.embedding_model
         t0 = time.perf_counter()
         # ---- phase A -------------------------------------------------------------
-        if self.vocab.normalize_nfc:      # real tokenizer files only (pretrained.py)
-            rows = _nfc_rows(rows)
+        rows = normalize_rows(rows, self.vocab)
         data, off = rows_to_blob(rows)
         n_rows, n_bytes = len(off) - 1, int(off[-1])
         if n_rows == 0:
@@ -728,8 +749,7 @@ def _infer_one_call(self, rows, system_prompt: Optional[str] = None,
     its three phases with CUDA events on the engine's stream: stats["t_h2d_ms"] (rows -> HBM),
     stats["t_device_ms"] (tokenise -> prefill/decode -> detokenise, HBM to HBM) and
     stats["t_d2h_ms"]."""
-    if self.vocab.normalize_nfc:
-        rows = _nfc_rows(rows)
+    rows = normalize_rows(rows, self.vocab)
     t0 = time.perf_counter()
     data, off = rows_to_blob(rows)
     n_rows = len(off) - 1

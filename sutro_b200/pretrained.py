@@ -98,7 +98,8 @@ def load_tokenizer_json(path: str, family: str, vocab_size: Optional[int] = None
         # for entries whose merges build something else: list those, with the sequence their
         # merges do build — the GPU tokenizer replaces exactly those sequences (two byte strings
         # never merge to the same tokens, so the replacement is exact).
-        rank = {pair: (i, merged_ids[i]) for i, pair in reversed(list(enumerate(merges)))}
+        # a pair listed twice ranks at its last occurrence, as in `tokenizers`
+        rank = {pair: (i, merged_ids[i]) for i, pair in enumerate(merges)}
         word_overrides = []
         for e, tb in enumerate(token_bytes):
             if len(tb) < 2:

@@ -117,14 +117,15 @@ def infer_frame_sharded(engine, rows=None, src: int = 0, balance: str = "bytes",
     Returns on `src` a dict(outputs | embeddings, stats, t_resident_s, t_results_resident_s,
     t_total_s); None on the other ranks.  With world size 1 (or no process group) the same
     code runs without the collectives.  `engine` needs `.device`, `.spec.embedding_model`,
-    `rows_select(...)` and `run_blob_dev(...)` (LocalEngine; a CPU stand-in in the gloo tests)."""
+    `rows_select(...)` and `run_blob_dev(...)` (LocalEngine; a CPU stand-in in the gloo tests);
+    its `.vocab`, when it has one, decides whether `src` NFC-normalises the rows first."""
     import time
 
     import numpy as np
     import torch
     import torch.distributed as dist
 
-    from .engine import blob_to_rows, rows_to_blob
+    from .engine import blob_to_rows, normalize_rows, rows_to_blob
     if balance not in ("rows", "bytes"):
         raise ValueError("balance must be 'rows' or 'bytes'")
     multi = dist.is_initialized() and dist.get_world_size() > 1
@@ -143,7 +144,7 @@ def infer_frame_sharded(engine, rows=None, src: int = 0, balance: str = "bytes",
     if rank == src:
         if rows is None:
             raise ValueError("the source rank must pass the rows")
-        data, off = rows_to_blob(rows)
+        data, off = rows_to_blob(normalize_rows(rows, getattr(engine, "vocab", None)))
         n_rows, n_bytes = len(off) - 1, int(off[-1])
         hdr = torch.tensor([n_rows, n_bytes], dtype=torch.int64, device=dev)
         d_text = torch.from_numpy(np.ascontiguousarray(data)).to(dev) if n_bytes else \

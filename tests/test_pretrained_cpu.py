@@ -170,6 +170,48 @@ def test_real_pretokenizer_patterns_and_normalizers(tmp_path):
         PT.load_tokenizer_json(path, "qwen3")
     from sutro_b200.engine import _nfc_rows
     assert _nfc_rows(["é", None, "plain", 3]) == ["é", None, "plain", 3]
+    import pandas as pd
+    import pyarrow as pa
+    from sutro_b200.engine import normalize_rows
+    # every input form the entry points accept comes out composed; without the flag, untouched
+    rows = ["e\u0301", None, "A\u030a", "\u1100\u1161\u11a8"]
+    want = ["\u00e9", None, "\u00c5", "\uac01"]
+    assert normalize_rows(rows, loaded) == want
+    assert normalize_rows(tuple(rows), loaded) == want
+    assert normalize_rows(pd.Series(rows[2:]), loaded) == want[2:]
+    assert normalize_rows(pa.array(rows), loaded).to_pylist() == want
+    assert normalize_rows(pa.chunked_array([rows[:1], rows[1:]]), loaded).to_pylist() == want
+    assert normalize_rows(pa.array(rows, type=pa.large_string()).slice(2),
+                          loaded).to_pylist() == want[2:]
+    ascii_col = pa.array(["plain", None])
+    assert normalize_rows(ascii_col, loaded) is ascii_col
+    import dataclasses
+    assert normalize_rows(rows, dataclasses.replace(loaded, normalize_nfc=False)) is rows
+    assert normalize_rows(rows, None) is rows
+
+
+def test_duplicate_merges_rank_at_their_last_entry(tmp_path):
+    """A merge listed twice takes the rank of its last entry in `tokenizers` (the merge map is
+    filled in list order); the loader and the oracle do the same."""
+    from tokenizers import Tokenizer
+    v = VB.build_vocab("qwen3", 2048, seed=0, n_trained=600)
+    path = str(tmp_path / "tokenizer.json")
+    gpt2_ordered_tokenizer(v).save(path)
+    tj = json.load(open(path))
+    tj["model"]["ignore_merges"] = True
+    json.dump(tj, open(path, "w"))
+    plain = Tokenizer.from_file(path)
+    tj["model"]["merges"] = tj["model"]["merges"] + tj["model"]["merges"][:60]
+    json.dump(tj, open(path, "w"))
+    hf = Tokenizer.from_file(path)
+    loaded = PT.load_tokenizer_json(path, "qwen3")
+    ref = RefTokenizer(loaded)
+    changed = 0
+    for text in TEXTS + ROWS_TXT + override_texts(loaded):
+        want = hf.encode(text, add_special_tokens=False).ids
+        assert loaded.to_real_ids(ref.encode(text)) == want, repr(text)
+        changed += want != plain.encode(text, add_special_tokens=False).ids
+    assert changed >= 3       # the demoted merges do change the tokenization
 
 
 def ignore_merges_vocab(tmp_path, family="llama"):

@@ -74,8 +74,9 @@ class TokenFSM:
     def enable_jump_forward(self, tokenizer) -> bool:
         """tokenizer: oracle RefTokenizer.  Sets `forced_prefix` (token ids every output starts
         with), moves `start` past it, and fills `tails[state]` (token ids of a continuation
-        that is forced up to a final state).  Returns False when the whole output is forced
-        (then nothing is enabled, like the engine)."""
+        that is forced up to a final state).  Returns False when the whole output is forced, or
+        when a forced string is not valid UTF-8 (a tail that starts inside a multi-byte
+        character has no text to encode); then nothing is enabled, like the engine."""
         prefix, after = self._forced(self.dfa.start)
         tails = {}
         for s in range(self.dfa.n_states):
@@ -84,9 +85,14 @@ class TokenFSM:
                 tails[s] = run
         if self.dfa.final[after] or after in tails:
             return False
-        self.forced_prefix = tokenizer.encode(prefix.decode("utf-8"))
+        try:
+            texts = {s: b.decode("utf-8") for s, b in tails.items()}
+            prefix_text = prefix.decode("utf-8")
+        except UnicodeDecodeError:
+            return False
+        self.forced_prefix = tokenizer.encode(prefix_text)
         self.start = after
-        self.tails = {s: tokenizer.encode(b.decode("utf-8")) for s, b in tails.items()}
+        self.tails = {s: tokenizer.encode(t) for s, t in texts.items()}
         return True
 
 
@@ -105,6 +111,8 @@ def validates(instance: Any, schema: Dict[str, Any], root=None) -> bool:
     sch = _resolve(root, schema)
     if sch is True or sch == {}:
         return True
+    if sch is False:
+        return False
     if "const" in sch:
         return instance == sch["const"]
     if "enum" in sch:
@@ -135,9 +143,11 @@ def validates(instance: Any, schema: Dict[str, Any], root=None) -> bool:
     if t == "null":
         return instance is None
     if t == "array":
+        pre = sch.get("prefixItems", [])
         return (isinstance(instance, list) and len(instance) >= sch.get("minItems", 0)
                 and len(instance) <= sch.get("maxItems", 1 << 30)
-                and all(validates(x, sch.get("items", {}), root) for x in instance))
+                and all(validates(x, pre[i] if i < len(pre) else sch.get("items", {}), root)
+                        for i, x in enumerate(instance)))
     return False
 
 

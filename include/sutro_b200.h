@@ -35,7 +35,8 @@ int sb200_device_info(int* sm_count, int* cc_major, int* cc_minor, size_t* total
 
 /* ------------------------------------------------------------------------
  * Kernel-level entry points (used by the parity tests; the engine calls the
- * same launchers internally).  Shapes are in elements, tensors are row-major.
+ * same launchers internally, one kernel per step).  Shapes are in elements,
+ * tensors are row-major.
  * ---------------------------------------------------------------------- */
 
 /* epilogue selectors for sb200_gemm_bf16_tn */
@@ -85,15 +86,17 @@ int sb200_attn_decode(const void* qkv, void* out, const void* kv_layer, const in
                       int max_pages, const int32_t* row_slot, const int32_t* ctx_len, int B, int hq,
                       int hkv, float scale, void* stream);
 
-/* test hook: 0 = automatic choice, 1 = 4-warps-per-pair split kernel, 2 = warp-per-pair */
+/* Kept for callers of the first ABI version: does nothing.  sb200_attn_decode has one kernel. */
 void sb200_attn_decode_force_variant(int v);
 
-/* K3: causal varlen prefill attention over the paged cache.  As for decode, the V values of the
- * slots past a sequence's last token in its last page must be finite. */
+/* Kept for callers of the first ABI version: the library has no paged prefill attention, so
+ * this returns -1.  An unsupported GQA group is reported as by the other attention entry
+ * points; otherwise sb200_last_error() names sb200_attn_prefill_dense. */
 int sb200_attn_prefill(const void* qkv, void* out, const void* kv_layer, const int32_t* page_table,
                        int max_pages, const int32_t* work, int n_work, const int32_t* seq_slot,
                        const int32_t* seq_q_start, const int32_t* seq_q_len,
                        const int32_t* seq_past, int hq, int hkv, float scale, void* stream);
+/* query tokens per work item of sb200_attn_prefill_dense: 128 / (hq / hkv) */
 int sb200_attn_prefill_q_tile(int hq, int hkv);
 
 /* K3 on wgmma tensor cores (the engine's prefill path): causal varlen attention over DENSE

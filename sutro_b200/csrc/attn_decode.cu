@@ -2,18 +2,19 @@
 //
 // HBM-bound: per generated token each sequence streams its whole K/V history
 // once (ctx_len x 2 x hkv x 256 B per layer).  Design:
-//   * grid = (kv_head, sequence); the G = hq/hkv query heads that share a KV
-//     head are processed together so K/V are read from HBM exactly once (GQA).
-//   * 4 warps per CTA; warp w owns KV pages w, w+4, ...  Each warp runs its own
-//     kStages-deep ring of 8 KiB stages filled by cp.async.bulk (UBLKCP): one
-//     lane issues a single flat 8 KiB copy per page (K tile + V tile of one
-//     head are contiguous in the pool), completion arrives on an mbarrier.
+//   * one WARP per (sequence, kv head) pair, 4 pairs per CTA; the G = hq/hkv
+//     query heads that share a KV head are processed together so K/V are read
+//     from HBM exactly once (GQA).
+//   * each warp streams its pair's pages through a private kDecStages-deep ring
+//     of 8 KiB stages filled by cp.async.bulk (UBLKCP): one lane issues a single
+//     flat 8 KiB copy per page (K tile + V tile of one head are contiguous in
+//     the pool), completion arrives on an mbarrier.
 //   * The pool stores tiles pre-swizzled (kernels.h), so the flat copy lands in
 //     shared memory bank-conflict-free for ldmatrix / ldmatrix.trans.
 //   * S = Q K^T and O += P V run on mma.sync m16n8k16 (bf16 in, fp32 acc) with
 //     the G query heads as the (zero-padded) M rows; online softmax uses
-//     quad-level warp shuffles; the 4 warps' partial (m, l, O) are merged
-//     through shared memory at the end.
+//     quad-level warp shuffles; the warp normalises and writes its output
+//     itself: no cross-warp merge and no block-wide barrier.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -25,10 +26,9 @@ constexpr int kDecWarps = 4;
 constexpr int kDecStages = 3;
 constexpr int kStageBytes = 2 * kTileBytes;  // K tile + V tile = 8 KiB
 constexpr int kDecSmem = kDecWarps * kDecStages * kStageBytes + 1024;
-int g_variant = 0;  // attn_decode_force_variant: 0 auto (the warp kernel), 1 split, 2 warp
 
-// Both kernels give each warp a private ring of kDecStages stages of kStageBytes (`ring`) with
-// one mbarrier per stage (`bars`); a stage holds one page.
+// Each warp owns a private ring of kDecStages stages of kStageBytes (`ring`) with one mbarrier
+// per stage (`bars`); a stage holds one page.
 SB_DEVICE void ring_init(uint64_t* bars, int lane) {
   if (lane == 0) {
 #pragma unroll
@@ -132,110 +132,6 @@ SB_DEVICE void decode_tile(uint32_t ks, const uint32_t (&qa)[8][2], int tile, in
 
 template <int G>
 __global__ void __launch_bounds__(kDecWarps * 32)
-attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out,
-                   const __nv_bfloat16* __restrict__ kv_layer,
-                   const int32_t* __restrict__ page_table, int max_pages,
-                   const int32_t* __restrict__ row_slot, const int32_t* __restrict__ ctx_len,
-                   int hq, int hkv, float scale_log2) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>(
-      (reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~static_cast<uintptr_t>(127));
-  __shared__ uint64_t full_bar[kDecWarps][kDecStages];
-  __shared__ float red_m[kDecWarps][8];
-  __shared__ float red_l[kDecWarps][8];
-
-  const int kvh = blockIdx.x;
-  const int b = blockIdx.y;
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int slot = row_slot[b];
-  const int L = ctx_len[b];
-  const int n_tiles = (L + kPageTokens - 1) / kPageTokens;
-  const int32_t* pt = page_table + static_cast<size_t>(slot) * max_pages;
-
-  uint8_t* my_smem = smem + warp * kDecStages * kStageBytes;
-  ring_init(full_bar[warp], lane);
-
-  // prologue: fill the ring
-  if (lane == 0) {
-#pragma unroll
-    for (int s = 0; s < kDecStages; ++s) {
-      const int tile = warp + s * kDecWarps;
-      if (tile < n_tiles) issue_page(kv_layer, pt[tile], hkv, kvh, my_smem, full_bar[warp], s);
-    }
-  }
-
-  const int qr = lane >> 2;
-  uint32_t qa[8][2];
-  load_q<G>(qkv, b, kvh, hq, hkv, lane, qa);
-
-  float o[16][2];
-#pragma unroll
-  for (int i = 0; i < 16; ++i) o[i][0] = o[i][1] = 0.f;
-  float m_run = -INFINITY, l_run = 0.f;
-
-  int it = 0;
-  for (int tile = warp; tile < n_tiles; tile += kDecWarps, ++it) {
-    const int stage = it % kDecStages;
-    const uint32_t phase = (it / kDecStages) & 1;
-    mbar_wait(smem_u32(&full_bar[warp][stage]), phase);
-    decode_tile(smem_u32(my_smem + stage * kStageBytes), qa, tile, L, scale_log2, lane, o, m_run,
-                l_run);
-
-    // ---- refill this stage with the tile kStages iterations ahead ----
-    __syncwarp();
-    const int next = tile + kDecStages * kDecWarps;
-    if (lane == 0 && next < n_tiles) {
-      fence_proxy_async_smem();  // generic-proxy reads above vs async-proxy write below
-      issue_page(kv_layer, pt[next], hkv, kvh, my_smem, full_bar[warp], stage);
-    }
-  }
-
-  // ---- merge the 4 warps' partial results ----
-  __syncthreads();  // all bulk copies consumed; stage memory is reusable as scratch
-  float* o_part = reinterpret_cast<float*>(smem) + warp * 8 * kHeadDim;  // [8][128] per warp
-  if ((lane & 3) == 0) {
-    red_m[warp][qr] = m_run;
-    red_l[warp][qr] = l_run;
-  }
-#pragma unroll
-  for (int nt = 0; nt < 16; ++nt) {
-    float2* dst = reinterpret_cast<float2*>(o_part + qr * kHeadDim + nt * 8 + 2 * (lane & 3));
-    *dst = make_float2(o[nt][0], o[nt][1]);
-  }
-  __syncthreads();
-  {
-    const int dim = threadIdx.x;  // 128 threads == 128 dims
-    const float* o_all = reinterpret_cast<const float*>(smem);
-#pragma unroll
-    for (int r = 0; r < G; ++r) {
-      float M = -INFINITY;
-#pragma unroll
-      for (int w = 0; w < kDecWarps; ++w) M = fmaxf(M, red_m[w][r]);
-      float num = 0.f, den = 0.f;
-#pragma unroll
-      for (int w = 0; w < kDecWarps; ++w) {
-        const float mw = red_m[w][r];
-        const float wgt = (mw == -INFINITY) ? 0.f : exp2f((mw - M) * scale_log2);
-        num += wgt * o_all[(w * 8 + r) * kHeadDim + dim];
-        den += wgt * red_l[w][r];
-      }
-      out[static_cast<size_t>(b) * hq * kHeadDim + (kvh * G + r) * kHeadDim + dim] =
-          __float2bfloat16_rn(num / den);
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------
-// Throughput variant: one WARP per (sequence, kv head).  When the batch offers at least a
-// few (sequence, kv head) pairs per resident warp there is no reason to split one pair
-// across warps: each warp streams its pair's pages through a private 3-stage ring and
-// writes the normalised output itself — no cross-warp merge, no __syncthreads, and the
-// page-table / Q-load / pipeline-fill latency is paid once per pair instead of once per
-// two or three tiles.
-// ---------------------------------------------------------------------------
-template <int G>
-__global__ void __launch_bounds__(kDecWarps * 32)
 attn_decode_warp_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out,
                         const __nv_bfloat16* __restrict__ kv_layer,
                         const int32_t* __restrict__ page_table, int max_pages,
@@ -283,7 +179,7 @@ attn_decode_warp_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __
     __syncwarp();
     const int next = tile + kDecStages;
     if (lane == 0 && next < n_tiles) {
-      fence_proxy_async_smem();
+      fence_proxy_async_smem();  // generic-proxy reads above vs async-proxy write below
       issue_page(kv_layer, pt[next], hkv, kvh, my_smem, full_bar[warp], stage);
     }
   }
@@ -306,29 +202,18 @@ int launch(const void* qkv, void* out, const void* kv_layer, const int32_t* page
   auto* o = static_cast<__nv_bfloat16*>(out);
   auto* kv = static_cast<const __nv_bfloat16*>(kv_layer);
   const float scale_log2 = scale * 1.4426950408889634f;
-  // The warp-per-(sequence, kv head) kernel is the only one the engine uses: which kernel
-  // runs must not depend on the batch size, or a row's greedy tokens would depend on its
-  // neighbours (the two kernels merge partial softmaxes in different orders).  The 4-warp
-  // split kernel stays for explicit requests (tests, latency experiments).
-  if (g_variant != 1) {
-    auto kern = attn_decode_warp_kernel<G>;
-    SB_SET_MAX_SMEM(kern, kDecSmem);
-    const int n_pairs = B * hkv;
-    kern<<<(n_pairs + kDecWarps - 1) / kDecWarps, kDecWarps * 32, kDecSmem, stream>>>(
-        q, o, kv, page_table, max_pages, row_slot, ctx_len, n_pairs, hq, hkv, scale_log2);
-  } else {
-    auto kern = attn_decode_kernel<G>;
-    SB_SET_MAX_SMEM(kern, kDecSmem);
-    kern<<<dim3(hkv, B), kDecWarps * 32, kDecSmem, stream>>>(
-        q, o, kv, page_table, max_pages, row_slot, ctx_len, hq, hkv, scale_log2);
-  }
+  // One kernel for every batch size: a kernel chosen by the batch would make a row's greedy
+  // tokens depend on its neighbours.
+  auto kern = attn_decode_warp_kernel<G>;
+  SB_SET_MAX_SMEM(kern, kDecSmem);
+  const int n_pairs = B * hkv;
+  kern<<<(n_pairs + kDecWarps - 1) / kDecWarps, kDecWarps * 32, kDecSmem, stream>>>(
+      q, o, kv, page_table, max_pages, row_slot, ctx_len, n_pairs, hq, hkv, scale_log2);
   SB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
 
 }  // namespace
-
-void attn_decode_force_variant(int v) { g_variant = v; }
 
 int attn_decode(const void* qkv, void* out, const void* kv_layer, const int32_t* page_table,
                 int max_pages, const int32_t* row_slot, const int32_t* ctx_len, int B, int hq,

@@ -6,8 +6,7 @@
 // activation buffer next to q, and the shared prefix's K/V are kept per layer in a small
 // dense side buffer.  Dense rows are what TMA wants: every operand tile below is one or a
 // few cp.async.bulk.tensor boxes that land in shared memory already in the wgmma canonical
-// 128-byte-swizzled layout.  (The paged cache is still written by the epilogue — decode reads
-// it — and attn_prefill.cu remains the general paged-KV path for callers outside the engine.)
+// 128-byte-swizzled layout.  (The paged cache is still written by the epilogue: decode reads it.)
 //
 // Work item = (sequence, kv head, q tile).  A q tile packs QT = 128/G consecutive tokens x
 // the G query heads of the kv head into 128 rows (row = token*G + head), so K/V are read once
@@ -401,6 +400,8 @@ int launch_tc(const TcMaps& m, void* out, const int32_t* items, int n_items, con
 }
 
 }  // namespace
+
+int attn_prefill_q_tile(int hq, int hkv) { return 128 / (hq / hkv); }
 
 int attn_prefill_dense(const void* qkv, int t_rows, void* out, const void* prefix_kv,
                        int prefix_rows, int n_layers, int layer, const int32_t* items, int n_items,

@@ -94,14 +94,18 @@ int sb200_attn_decode(const void* qkv, void* out, const void* kv_layer, const in
                      scale, STREAM(stream));
 }
 
-void sb200_attn_decode_force_variant(int v) { attn_decode_force_variant(v); }
+// Kept for callers of ABI version 1 (see the header).
+void sb200_attn_decode_force_variant(int) {}
 
-int sb200_attn_prefill(const void* qkv, void* out, const void* kv_layer, const int32_t* page_table,
-                       int max_pages, const int32_t* work, int n_work, const int32_t* seq_slot,
-                       const int32_t* seq_q_start, const int32_t* seq_q_len,
-                       const int32_t* seq_past, int hq, int hkv, float scale, void* stream) {
-  return attn_prefill(qkv, out, kv_layer, page_table, max_pages, work, n_work, seq_slot,
-                      seq_q_start, seq_q_len, seq_past, hq, hkv, scale, STREAM(stream));
+int sb200_attn_prefill(const void*, void*, const void*, const int32_t*, int, const int32_t*, int,
+                       const int32_t*, const int32_t*, const int32_t*, const int32_t*, int hq,
+                       int hkv, float, void*) {
+  // the GQA group is still rejected as the other attention launchers reject it
+  return dispatch_gqa("attn_prefill", hq, hkv, [](auto) {
+    set_last_error("sb200_attn_prefill: the library has no paged prefill attention; use "
+                   "sb200_attn_prefill_dense");
+    return -1;
+  });
 }
 
 int sb200_attn_prefill_q_tile(int hq, int hkv) { return attn_prefill_q_tile(hq, hkv); }

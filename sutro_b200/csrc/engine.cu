@@ -12,7 +12,6 @@
 // workspaces sized for max(max_prefill_tokens, max_slots) tokens, a logits
 // chunk, the page table and the per-slot decode state.
 #include <algorithm>
-#include <cstdlib>
 #include <functional>
 #include <string>
 #include <vector>
@@ -219,10 +218,6 @@ struct Engine {
   Profiler prof;
   double gemm_flops = 0, attn_decode_bytes = 0;
   int device = 0;
-  bool fuse_qkv = true;  // SB200_FUSE_QKV=0 keeps the separate rope_kv_write kernel (A/B tests)
-  // wgmma prefill attention over dense K/V (attn_prefill_tc.cu); SB200_PREFILL_TC=0 falls
-  // back to the paged mma.sync kernel (A/B tests)
-  bool prefill_tc = true;
   bf16* prefix_kv = nullptr;  // [n_layers][prefix_rows][2*hkv*128]: dense K|V of the shared prefix
   int prefix_rows = 0;
   bool fill_prefix = false;   // this forward pass is the prefix prefill: keep its K/V
@@ -255,8 +250,6 @@ struct Engine {
     q_tile = attn_prefill_q_tile(c.n_q_heads, c.n_kv_heads);
     num_pages = c.num_pages;
     layer_stride = num_pages * kv_page_elems(c.n_kv_heads);
-    if (const char* e = getenv("SB200_FUSE_QKV")) fuse_qkv = e[0] != '0';
-    if (const char* e = getenv("SB200_PREFILL_TC")) prefill_tc = e[0] != '0';
     SB_CUDA_CHECK(cudaGetDevice(&device));
     SB_CUDA_CHECK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
     const size_t T = t_max, S = c.max_slots + 2;  // +prefix slot, +dummy slot
@@ -298,8 +291,7 @@ struct Engine {
   // prefill: attention over (cached prefix | new tokens) per sequence;
   // decode : one token per sequence against its paged history.
   int forward(int T, bool prefill, const int32_t* d_work, int n_work,
-              const int32_t* d_seq_slot, const int32_t* d_seq_q_start, const int32_t* d_seq_q_len,
-              const int32_t* d_seq_past) {
+              const int32_t* d_seq_q_start, const int32_t* d_seq_q_len, const int32_t* d_seq_past) {
     const auto& c = cfg;
     const float scale = 1.0f / sqrtf(static_cast<float>(kHeadDim));
     auto gemm = [&](const void* a, const void* wt, void* d, const void* r, int M, int N, int K,
@@ -310,21 +302,14 @@ struct Engine {
     SB_K(SB200_KC_EMBED, embed_gather(tok_ids, w.embed, x, T, c.d_model, stream));
     for (int l = 0; l < c.n_layers; ++l) {
       SB_K(SB200_KC_NORM, rmsnorm(x, ln1[l], h, T, c.d_model, c.rms_eps, stream));
-      if (fuse_qkv) {
-        // K1+K5 fused: q/k-norm, RoPE and the paged K/V write happen in the GEMM epilogue
-        QkvEpiArgs qa{tok_pos, tok_slot, page_table, max_pages, kv_layer(l), w.rope_cos,
-                      w.rope_sin, qn[l], kn[l], c.n_q_heads, c.n_kv_heads, c.rms_eps,
-                      (prefill && prefill_tc) ? 1 : 0};
-        gemm_flops += 2.0 * T * qkv_dim * c.d_model;
-        SB_K(SB200_KC_GEMM, gemm_bf16_tn(h, t_max, wqkv[l], qkv, nullptr, T, qkv_dim, c.d_model,
-                                         qkv_dim, EPI_QKV_ROPE, 0, stream, &qa));
-      } else {
-        SB_K(SB200_KC_GEMM, gemm(h, wqkv[l], qkv, nullptr, T, qkv_dim, c.d_model, qkv_dim,
-                                 EPI_STORE_BF16));
-        SB_K(SB200_KC_ROPE, rope_kv_write(qkv, qn[l], kn[l], w.rope_cos, w.rope_sin, tok_slot,
-                                          tok_pos, page_table, max_pages, kv_layer(l), T,
-                                          c.n_q_heads, c.n_kv_heads, c.rms_eps, stream));
-      }
+      // K1+K5 fused: q/k-norm, RoPE and the paged K/V write happen in the GEMM epilogue; in
+      // prefill it also leaves K/V in their qkv columns for the dense prefill attention
+      QkvEpiArgs qa{tok_pos, tok_slot, page_table, max_pages, kv_layer(l), w.rope_cos,
+                    w.rope_sin, qn[l], kn[l], c.n_q_heads, c.n_kv_heads, c.rms_eps,
+                    prefill ? 1 : 0};
+      gemm_flops += 2.0 * T * qkv_dim * c.d_model;
+      SB_K(SB200_KC_GEMM, gemm_bf16_tn(h, t_max, wqkv[l], qkv, nullptr, T, qkv_dim, c.d_model,
+                                       qkv_dim, EPI_QKV_ROPE, 0, stream, &qa));
       if (prefill && fill_prefix && prefix_kv != nullptr) {
         // the shared prefix's K/V (k|v columns of its rows) go to the dense side buffer
         const size_t cols = 2ull * c.n_kv_heads * kHeadDim;
@@ -332,16 +317,11 @@ struct Engine {
                                         cols * sizeof(bf16), qkv + q_dim, qkv_dim * sizeof(bf16),
                                         cols * sizeof(bf16), T, cudaMemcpyDeviceToDevice, stream));
       }
-      if (prefill && prefill_tc) {
+      if (prefill) {
         SB_K(SB200_KC_ATTN_PREFILL,
              attn_prefill_dense(qkv, t_max, attn, prefix_kv, prefix_rows, c.n_layers, l, d_work,
                                 n_work, d_seq_q_start, d_seq_q_len, d_seq_past, c.n_q_heads,
                                 c.n_kv_heads, scale, stream));
-      } else if (prefill) {
-        SB_K(SB200_KC_ATTN_PREFILL,
-             attn_prefill(qkv, attn, kv_layer(l), page_table, max_pages, d_work, n_work,
-                          d_seq_slot, d_seq_q_start, d_seq_q_len, d_seq_past, c.n_q_heads,
-                          c.n_kv_heads, scale, stream));
       } else {
         SB_K(SB200_KC_ATTN_DECODE,
              attn_decode(qkv, attn, kv_layer(l), page_table, max_pages, row_slot, ctx_len, T,
@@ -612,7 +592,7 @@ int Engine::run(const sb200_job& job, sb200_job_stats* stats) {
           prefix_tail_page, d_copy);
     }
     SB_CUDA_CHECK(cudaGetLastError());
-    if (forward(T, true, d_work, n_work, d_misc, d_misc + (S + 2), d_misc + 2 * (S + 2),
+    if (forward(T, true, d_work, n_work, d_misc + (S + 2), d_misc + 2 * (S + 2),
                 d_misc + 3 * (S + 2)))
       return -1;
     if (!sample) return 0;
@@ -648,7 +628,7 @@ int Engine::run(const sb200_job& job, sb200_job_stats* stats) {
     h_seqs[0] = SeqInit{prefix_slot, -1, 0, prefix_cached, 0, 0, 1, -1};
     std::fill(h_pt, h_pt + max_pages, 0);
     std::copy(prefix_pages.begin(), prefix_pages.end(), h_pt);
-    if (prefill_tc && prefix_cached > prefix_rows) {
+    if (prefix_cached > prefix_rows) {
       cudaFree(prefix_kv);
       prefix_kv = nullptr;
       prefix_rows = 0;
@@ -801,7 +781,7 @@ int Engine::run(const sb200_job& job, sb200_job_stats* stats) {
     const int prc = prepare_decode(row_slot, slot_next_tok, slot_pos, tok_ids, tok_pos, tok_slot,
                                    ctx_len, B, stream);
     prof.end();
-    if (prc || forward(B, false, nullptr, 0, nullptr, nullptr, nullptr, nullptr) ||
+    if (prc || forward(B, false, nullptr, 0, nullptr, nullptr, nullptr) ||
         head_and_sample(B, nullptr, row_slot, job, has_fsm)) {
       rc = -1;
       break;

@@ -31,7 +31,6 @@
 // TMA clips every store and residual load at the tensor map's dims (M rows, N or N/2 columns),
 // so rows >= M and columns past N are never written.
 #include <algorithm>
-#include <cstdlib>
 #include <mutex>
 #include <unordered_map>
 
@@ -629,11 +628,6 @@ int l2_bytes() {
 // streamed: there the group takes as many row-tiles as keep its A slab (rows x K bf16) within
 // ~40 % of the L2, so A is read from HBM once and W once per group.
 int raster_group(int tile_rows, int N, int K) {
-  static const int forced = [] {   // SB200_GEMM_GM: fixes the group size (tuning experiments)
-    const char* e = getenv("SB200_GEMM_GM");
-    return e ? atoi(e) : 0;
-  }();
-  if (forced > 0) return forced;
   const long l2 = l2_bytes();
   if (static_cast<long>(N) * K * 2 <= l2 / 2) return 2;
   const long slab = l2 * 2 / 5;

@@ -96,17 +96,7 @@ int attn_decode(const void* qkv, void* out, const void* kv_layer, const int32_t*
                 int max_pages, const int32_t* row_slot, const int32_t* ctx_len, int B, int hq,
                 int hkv, float scale, cudaStream_t stream);
 
-void attn_decode_force_variant(int v);  // 0 auto, 1 split kernel, 2 warp-per-pair kernel
-
-// K3 — causal prefill attention over the paged cache (varlen batch).
-// work: [n_work] {seq, q_tile_start}; per-seq arrays are indexed by seq.
-int attn_prefill(const void* qkv, void* out, const void* kv_layer, const int32_t* page_table,
-                 int max_pages, const int32_t* work, int n_work, const int32_t* seq_slot,
-                 const int32_t* seq_q_start, const int32_t* seq_q_len, const int32_t* seq_past,
-                 int hq, int hkv, float scale, cudaStream_t stream);
-int attn_prefill_q_tile(int hq, int hkv);
-
-// K3 (wgmma) — causal prefill attention over DENSE K/V: new tokens' K/V are the k/v columns
+// K3 — causal prefill attention over DENSE K/V: new tokens' K/V are the k/v columns
 // of the qkv buffer itself (post-norm/RoPE, written by the fused QKV epilogue), the shared
 // prefix's K/V live in prefix_kv[n_layers][prefix_rows][2*hkv*128] (K heads | V heads).
 // items: [n_items] {seq, q_tile_start} with q tile = attn_prefill_q_tile(); every sequence
@@ -115,6 +105,7 @@ int attn_prefill_dense(const void* qkv, int t_rows, void* out, const void* prefi
                        int prefix_rows, int n_layers, int layer, const int32_t* items, int n_items,
                        const int32_t* seq_q_start, const int32_t* seq_q_len,
                        const int32_t* seq_past, int hq, int hkv, float scale, cudaStream_t stream);
+int attn_prefill_q_tile(int hq, int hkv);  // query tokens per work item: 128 / G
 
 // bf16 tensor map, 128-byte swizzle, rank 2..5 (gemm_wgmma.cu)
 int encode_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims,

@@ -65,6 +65,8 @@ class JobC(C.Structure):
                 ("out_cum_logprob_dev", C.c_void_p), ("row_ids_dev", C.c_void_p)]
 
 
+# indexed by SB200_KC_*; "rope" stays in the stats layout but counts 0: RoPE and the K/V write
+# run in the QKV GEMM's epilogue, counted under "gemm"
 KERNEL_CLASSES = ["gemm", "attn_decode", "attn_prefill", "norm", "rope", "sample", "embed",
                   "other"]
 _STAT_INTS = ("rows_done", "input_tokens", "prefill_tokens", "decode_tokens", "prefill_steps",

@@ -48,8 +48,9 @@ from sutro_b200 import vocab as VB
 PAGE = 16
 HD = 128
 EPI_RESIDUAL_BF16, EPI_SWIGLU_BF16, EPI_STORE_F32 = 1, 2, 3
-# switches that move the engine off the path replayed here
-ENGINE_SWITCHES = ("SB200_FUSE_QKV", "SB200_PREFILL_TC", "SB200_QKV_DENSE")
+# switches that move the replay off the engine's path (SB200_QKV_DENSE=0: sb200_gemm_qkv_rope
+# skips the dense K/V copy that the replayed prefill attention reads)
+ENGINE_SWITCHES = ("SB200_QKV_DENSE",)
 
 
 @dataclass
@@ -76,8 +77,6 @@ class Replay:
         self.eng, self.spec, self.w, self.v = eng, eng.spec, eng.weights, eng.vocab
         self.dev = eng.device
         self.lib = L.lib()
-        # process-wide test hook of the decode attention: 0 is the engine's automatic choice
-        self.lib.sb200_attn_decode_force_variant(0)
         s = self.spec
         self.q_tile = self.lib.sb200_attn_prefill_q_tile(s.n_q_heads, s.n_kv_heads)
         self.max_pages = (s.max_position + PAGE - 1) // PAGE + 1

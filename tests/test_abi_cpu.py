@@ -70,6 +70,31 @@ def test_attention_launchers_reject_unsupported_gqa_groups(hq, hkv, msg):
         assert lib.sb200_last_error().decode() == f"{who}: {msg}"
 
 
+@pytest.mark.skipif(not os.path.exists(LIB), reason="library not built")
+def test_attn_prefill_stub_names_the_dense_kernel():
+    """sb200_attn_prefill stays in ABI version 1 without a kernel behind it: with a supported GQA
+    group it fails before any CUDA call, so this needs no GPU."""
+    lib = ctypes.CDLL(LIB)
+    lib.sb200_last_error.restype = ctypes.c_char_p
+    ints = (ctypes.c_int32 * 4)()
+    assert lib.sb200_attn_prefill(None, None, None, ints, 1, ints, 1, ints, ints, ints, ints, 32,
+                                  8, ctypes.c_float(1.0), None) == -1
+    assert lib.sb200_last_error().decode() == (
+        "sb200_attn_prefill: the library has no paged prefill attention; use "
+        "sb200_attn_prefill_dense")
+
+
+@pytest.mark.skipif(not os.path.exists(LIB), reason="library not built")
+def test_decode_force_variant_is_still_exported():
+    """sb200_attn_decode_force_variant stays in ABI version 1 as a no-op (one decode kernel)."""
+    lib = ctypes.CDLL(LIB)
+    fn = lib.sb200_attn_decode_force_variant
+    fn.restype = None
+    fn.argtypes = [ctypes.c_int]
+    for v in (0, 1, 2):
+        fn(v)
+
+
 def test_no_product_module_imports_the_oracle():
     pkg = os.path.join(ROOT, "sutro_b200")
     for dirpath, _, files in os.walk(pkg):

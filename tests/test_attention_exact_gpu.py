@@ -1,9 +1,8 @@
 """Attention kernels checked bit for bit where the math allows it, and against fp64 elsewhere.
 
-Covers the dense prefill attention (attn_prefill_tc.cu, the engine's prefill path), the paged
-prefill attention (attn_prefill.cu), both decode kernels (attn_decode.cu) and the fused QKV
-epilogue's dense K/V copy (gemm_wgmma.cu), all through the C ABI, at the four GQA group sizes and
-the engine's scale 1/sqrt(128):
+Covers the dense prefill attention (attn_prefill_tc.cu), the decode attention (attn_decode.cu)
+and the fused QKV epilogue's dense K/V copy (gemm_wgmma.cu), all through the C ABI, at the four
+GQA group sizes and the engine's scale 1/sqrt(128):
 
 1. Masked rows do not matter.  Every location a kernel may load but must not use (rows past a
    sequence's end inside a 32-row TMA box, prefix rows at or after `past`, other kv heads, other
@@ -68,7 +67,7 @@ def ulp_bf16(x):
 
 
 def error_bound(ref, mag):
-    """Per-element bound on |got - ref| for all three attention kernels.
+    """Per-element bound on |got - ref| for both attention kernels.
 
     ref = sum_j p_j v_j / sum_j p_j in fp64, mag = sum_j p_j |v_j| / sum_j p_j.  The kernels
     compute p_j in fp32 (up to a common factor: the dense kernel rescales lazily, so its P may
@@ -228,35 +227,15 @@ def run_dense(qkv, pre, prefix_rows, n_layers, layer, specs, hq, hkv):
     return out[:T].view(T, hq, HD)
 
 
-def run_paged(qkv, pool, pt, specs, hq, hkv):
-    """sb200_attn_prefill; sequence i lives in page-table row i.  -> [T, hq, 128]."""
-    q_start, T = starts(specs)
-    work = q_tiles(specs, hq, hkv)
-    out = torch.zeros(T, hq * HD, dtype=torch.bfloat16, device=DEV)
-    d_pt, d_work, d_slot = i32(pt), i32(work), i32(list(range(len(specs))))
-    d_qs, d_ql = i32(q_start), i32([n for _, n in specs])
-    d_past = i32([p for p, _ in specs])
-    L.check(L.lib().sb200_attn_prefill(
-        L.ptr(qkv), L.ptr(out), L.ptr(pool), L.ptr(d_pt), pt.shape[1], L.ptr(d_work),
-        len(work) // 2, L.ptr(d_slot), L.ptr(d_qs), L.ptr(d_ql), L.ptr(d_past), hq, hkv, SCALE,
-        L.current_stream()))
-    torch.cuda.synchronize()
-    return out.view(T, hq, HD)
-
-
-def run_decode(qkv, pool, pt, row_slot, ctx, hq, hkv, variant):
-    """sb200_attn_decode with the kernel variant forced (1: split, 2: warp per pair)."""
+def run_decode(qkv, pool, pt, row_slot, ctx, hq, hkv):
+    """sb200_attn_decode.  -> [B, hq, 128]."""
     B = qkv.shape[0]
     out = torch.zeros(B, hq * HD, dtype=torch.bfloat16, device=DEV)
     d_pt, d_rs, d_ctx = i32(pt), i32(row_slot), i32(ctx)
-    L.lib().sb200_attn_decode_force_variant(variant)
-    try:
-        L.check(L.lib().sb200_attn_decode(L.ptr(qkv), L.ptr(out), L.ptr(pool), L.ptr(d_pt),
-                                          pt.shape[1], L.ptr(d_rs), L.ptr(d_ctx), B, hq, hkv,
-                                          SCALE, L.current_stream()))
-        torch.cuda.synchronize()
-    finally:
-        L.lib().sb200_attn_decode_force_variant(0)
+    L.check(L.lib().sb200_attn_decode(L.ptr(qkv), L.ptr(out), L.ptr(pool), L.ptr(d_pt),
+                                      pt.shape[1], L.ptr(d_rs), L.ptr(d_ctx), B, hq, hkv, SCALE,
+                                      L.current_stream()))
+    torch.cuda.synchronize()
     return out.view(B, hq, HD)
 
 
@@ -434,69 +413,6 @@ def last_page_tails(pt, lens):
     return pages, slots
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("hq,hkv", HEADS, ids=HEAD_IDS)
-def test_paged_prefill_masked_slots_do_not_leak(hq, hkv):
-    G = hq // hkv
-    specs = [(37, 300), (0, 161), (5, 17), (64, 140), (0, 9)]
-    lens = [p + n for p, n in specs]
-    q_start, T = starts(specs)
-    torch.manual_seed(10 + G)
-    u = torch.randn(hkv, HD, device=DEV)
-    ks = [bf(torch.randn(l, hkv, HD, device=DEV)) for l in lens]
-    vs = [bf(torch.randn(l, hkv, HD, device=DEV)) for l in lens]
-    logical, pt, decoy_page, spare = paged_cache(ks, vs, seed=G)
-    qkv = queries(T, hq, hkv, u)
-
-    def run():
-        return run_paged(qkv, KV.pack_tile(logical), pt, specs, hq, hkv)
-
-    def unchanged(mod):
-        m = torch.ones(T, hq, dtype=torch.bool)
-        for s, (p, n) in enumerate(specs):
-            first = first_touched(mod, pt[s], p + n)
-            m[q_start[s]:q_start[s] + n] = (p + torch.arange(n))[:, None] < \
-                first.repeat_interleave(G)[None, :]
-        return m
-
-    base = run()
-    logical[spare] = float("nan")                 # referenced by no page-table entry
-    assert torch.equal(run(), base)
-    saved = logical.clone()
-    fresh = lambda: torch.zeros(logical.shape[0], hkv, PAGE, dtype=torch.bool)
-    # the decoy page every entry past a sequence's last page points at
-    mod = fresh()
-    paged_decoys(logical, u, mod, [decoy_page] * PAGE, list(range(PAGE)))
-    check_unchanged(run(), base, unchanged(fresh()), "page-table entries past the last page")
-    logical.copy_(saved)
-    # unused slots of each last page
-    mod = fresh()
-    paged_decoys(logical, u, mod, *last_page_tails(pt, lens))
-    check_unchanged(run(), base, unchanged(mod), "slots past the sequence end")
-    logical.copy_(saved)
-    # own positions after the causal frontier
-    for s, js in ((0, (15, 16, 17, 31, 32, 33, 127, 128, 129, 255, 256)), (3, (0, 1, 127, 128))):
-        for j in js:
-            pos = specs[s][0] + j
-            mod = fresh()
-            paged_decoys(logical, u, mod, int(pt[s, pos // PAGE]), pos % PAGE)
-            check_unchanged(run(), base, unchanged(mod), f"position {pos} of sequence {s}")
-            logical.copy_(saved)
-    # kv head 0's tiles of every page
-    if hkv > 1:
-        mod = fresh()
-        n_pg = logical.shape[0]
-        paged_decoys(logical, u, mod, torch.arange(n_pg).repeat_interleave(PAGE),
-                     torch.arange(PAGE).repeat(n_pg), kv_heads=[0])
-        check_unchanged(run(), base, unchanged(mod), "kv head 0")
-        logical.copy_(saved)
-    # every page of another slot
-    mod = fresh()
-    pages = pt[1, :(lens[1] + PAGE - 1) // PAGE]
-    paged_decoys(logical, u, mod, pages.repeat_interleave(PAGE), torch.arange(PAGE).repeat(len(pages)))
-    check_unchanged(run(), base, unchanged(mod), "pages of slot 1")
-
-
 def decode_case(lens, hq, hkv, share, seed):
     """Per-slot K/V (slots longer than `share` pages share those pages), queries for rows mapped
     to slots in reverse order."""
@@ -518,7 +434,7 @@ def decode_case(lens, hq, hkv, share, seed):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", [1, 2])
+@pytest.mark.parametrize("variant", [2])      # the warp-per-(sequence, kv head) kernel
 @pytest.mark.parametrize("hq,hkv", HEADS, ids=HEAD_IDS)
 def test_decode_masked_slots_do_not_leak(hq, hkv, variant):
     G = hq // hkv
@@ -529,7 +445,7 @@ def test_decode_masked_slots_do_not_leak(hq, hkv, variant):
     qkv = queries(len(lens), hq, hkv, u)
 
     def run():
-        return run_decode(qkv, KV.pack_tile(logical), pt, row_slot, ctx, hq, hkv, variant)
+        return run_decode(qkv, KV.pack_tile(logical), pt, row_slot, ctx, hq, hkv)
 
     def unchanged(mod):
         m = torch.ones(len(lens), hq, dtype=torch.bool)
@@ -667,42 +583,7 @@ def test_dense_prefill_pointer_is_exact(hq, hkv):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("hq,hkv", HEADS, ids=HEAD_IDS)
-def test_paged_prefill_pointer_is_exact(hq, hkv):
-    G = hq // hkv
-    specs = [(257, 260), (0, 300), (40, 1), (0, 33), (17, 129)]
-    lens = [p + n for p, n in specs]
-    q_start, T = starts(specs)
-    gen = torch.Generator().manual_seed(40 + G)
-    pq = PointerQueries(hq, hkv, seed=100 + G)
-    probe_at = []
-    for s, (p, n) in enumerate(specs):
-        edges = EDGES + ((p - 1, p) if p else ())
-        for t in range(n):
-            c = pq.add_row(p + t, edges + (p + t,), probe=t in (0, 15, 31, 127, n - 1))
-            if c is not None:
-                probe_at.append((s, p + t + 1, pq.probes[-1][1] // G, c))
-    ks = [torch.stack([kv_address(torch.arange(l), h) for h in range(hkv)], 1) for l in lens]
-    vs = [pointer_value(l, hkv, gen) for l in lens]
-    logical, pt, decoy_page, _ = paged_cache([bf(k) for k in ks], vs, seed=G)
-    for s, pos, h, c in probe_at:      # key right after the diagonal, if it has a page slot
-        if pos < lens[s] or pos % PAGE:
-            slot = logical[int(pt[s, pos // PAGE]), h, 0, pos % PAGE]
-            slot.copy_(bf(kv_address(pos % N_ADDR, h)[0]).to(DEV))
-            slot[64 + c] = D_PTR
-    logical[decoy_page, :, 0, :, 64:] = D_PTR     # every channel, past each last page
-    out = run_paged(qkv_rows(pq.q(), hkv), KV.pack_tile(logical), pt, specs, hq, hkv)
-    tgt = torch.tensor(pq.tgt)
-    want = torch.empty(T, hq, HD, dtype=torch.bfloat16)
-    for s, (p, n) in enumerate(specs):
-        blk = tgt[q_start[s]:q_start[s] + n]
-        want[q_start[s]:q_start[s] + n] = vs[s][blk, (torch.arange(hq) // G)[None, :]]
-    bad = (out != want.to(DEV)).any(-1).nonzero()
-    assert bad.numel() == 0, (len(bad), bad[:8].tolist())
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("variant", [1, 2])
+@pytest.mark.parametrize("variant", [2])      # the warp-per-(sequence, kv head) kernel
 @pytest.mark.parametrize("hq,hkv", HEADS, ids=HEAD_IDS)
 def test_decode_pointer_is_exact(hq, hkv, variant):
     """Targets at the edges and at L-1; three pages of shared prefix, rows mapped to slots in
@@ -731,8 +612,7 @@ def test_decode_pointer_is_exact(hq, hkv, variant):
         if l % PAGE:
             logical[int(pt[s, l // PAGE]), h, 0, l % PAGE, 64 + c] = D_PTR
     logical[decoy_page, :, 0, :, 64:] = D_PTR
-    out = run_decode(qkv_rows(pq.q(), hkv), KV.pack_tile(logical), pt, row_slot, ctx, hq, hkv,
-                     variant)
+    out = run_decode(qkv_rows(pq.q(), hkv), KV.pack_tile(logical), pt, row_slot, ctx, hq, hkv)
     tgt = torch.tensor(pq.tgt)
     want = torch.stack([vs[row_slot[b]][tgt[b], torch.arange(hq) // G] for b in range(B)])
     bad = (out != want.to(DEV)).any(-1).nonzero()
@@ -801,32 +681,10 @@ def test_dense_prefill_error_bound(case, hq, hkv, specs, gain, ramp):
     assert_within_bound(out, ref, mag, f"dense prefill {case}")
 
 
-PAGED_SPECS = [(0, 2049), (1000, 1025), (997, 129), (0, 15), (500, 145), (37, 31), (0, 289),
-               (1000, 127), (64, 129)]
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("hq,hkv", HEADS, ids=HEAD_IDS)
-def test_paged_prefill_error_bound(hq, hkv):
-    specs = PAGED_SPECS if hq == 32 else PAGED_SPECS[1:]
-    lens = [p + n for p, n in specs]
-    q_start, T = starts(specs)
-    torch.manual_seed(60 + hq + hkv)
-    ks = [bf(torch.randn(l, hkv, HD, device=DEV)) for l in lens]
-    vs = [bf(torch.randn(l, hkv, HD, device=DEV)) for l in lens]
-    qkv = bf(torch.randn(T, (hq + 2 * hkv) * HD, device=DEV))
-    logical, pt, _, _ = paged_cache(ks, vs, seed=hq)
-    out = run_paged(qkv, KV.pack_tile(logical), pt, specs, hq, hkv)
-    refs = [attn_ref64(qkv[q_start[s]:q_start[s] + n, :hq * HD].view(n, hq, HD), ks[s], vs[s],
-                       p + 1 + torch.arange(n), hkv) for s, (p, n) in enumerate(specs)]
-    assert_within_bound(out, torch.cat([r for r, _ in refs]), torch.cat([m for _, m in refs]),
-                        f"paged prefill G{hq // hkv}")
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("hq,hkv", HEADS, ids=HEAD_IDS)
 def test_decode_error_bound(hq, hkv):
-    """Contexts up to 4096 over hundreds of rows (256 at the real models' shape), both kernels."""
+    """Contexts up to 4096 over hundreds of rows (256 at the real models' shape)."""
     B = 256 if hq == 32 else 64
     g = torch.Generator().manual_seed(hq + hkv)
     fixed = [1, 15, 16, 17, 129, 2048, 4095, 4096]
@@ -839,9 +697,8 @@ def test_decode_error_bound(hq, hkv):
     refs = [attn_ref64(qkv[b:b + 1, :hq * HD].view(1, hq, HD), ks[s], vs[s], [ctx[b]], hkv)
             for b, s in enumerate(row_slot)]
     ref, mag = torch.cat([r for r, _ in refs]), torch.cat([m for _, m in refs])
-    for variant in (1, 2):
-        out = run_decode(qkv, pool, pt, row_slot, ctx, hq, hkv, variant)
-        assert_within_bound(out, ref, mag, f"decode variant {variant} G{hq // hkv}")
+    out = run_decode(qkv, pool, pt, row_slot, ctx, hq, hkv)
+    assert_within_bound(out, ref, mag, f"decode G{hq // hkv}")
 
 
 # --------------------------------------------------------------------------- 4. fused QKV epilogue

@@ -256,10 +256,9 @@ def test_gemm_qkv_rope_fused_matches_unfused(qk_norm, block_n):
 
 
 # --------------------------------------------------------------------------- attention
-@pytest.mark.parametrize("variant", [1, 2])   # 1: 4-warp split kernel, 2: warp-per-pair kernel
+@pytest.mark.parametrize("variant", [2])   # the warp-per-(sequence, kv head) kernel
 @pytest.mark.parametrize("hq,hkv", [(32, 8), (16, 8), (8, 8), (16, 2)])
 def test_attn_decode(hq, hkv, variant):
-    L.lib().sb200_attn_decode_force_variant(variant)
     torch.manual_seed(hq * 100 + hkv)
     lens = [1, 15, 16, 17, 63, 64, 65, 130, 257, 600]
     B = len(lens)
@@ -275,46 +274,10 @@ def test_attn_decode(hq, hkv, variant):
     L.check(L.lib().sb200_attn_decode(L.ptr(qkv), L.ptr(out), L.ptr(pool), L.ptr(pt), max_pages,
                                       L.ptr(row_slot), L.ptr(ctx), B, hq, hkv, scale, stream()))
     torch.cuda.synchronize()
-    L.lib().sb200_attn_decode_force_variant(0)
     refs = [attn_ref64(qkv[b:b + 1, :hq * KV.HD].view(1, hq, KV.HD), ks[B - 1 - b], vs[B - 1 - b],
                        [lens[B - 1 - b]], hkv) for b in range(B)]
     assert_within_bound(out, torch.cat([r for r, _ in refs]), torch.cat([m for _, m in refs]),
-                        f"decode variant {variant} {hq}/{hkv}")
-
-
-@pytest.mark.parametrize("hq,hkv", [(32, 8), (16, 8), (4, 4)])
-def test_attn_prefill(hq, hkv):
-    torch.manual_seed(hq + hkv)
-    # (past, new) per sequence: fresh prompts and prompts behind a cached prefix
-    specs = [(0, 1), (0, 16), (0, 17), (0, 100), (32, 5), (32, 70), (48, 200), (3, 33)]
-    n = len(specs)
-    ks = [bf(torch.randn(p + q, hkv, KV.HD, device=DEV)) for p, q in specs]
-    vs = [bf(torch.randn(p + q, hkv, KV.HD, device=DEV)) for p, q in specs]
-    pool, pt, max_pages = KV.build_cache(ks, vs, hkv, 200, DEV)
-    T = sum(q for _, q in specs)
-    qkv = bf(torch.randn(T, (hq + 2 * hkv) * KV.HD, device=DEV))
-    out = torch.zeros(T, hq * KV.HD, dtype=torch.bfloat16, device=DEV)
-    qt = L.lib().sb200_attn_prefill_q_tile(hq, hkv)
-    assert qt == 128 // (hq // hkv)
-    q_start, work, acc = [], [], 0
-    for i, (p, q) in enumerate(specs):
-        q_start.append(acc)
-        acc += q
-        for t0 in range(0, q, qt):
-            work += [i, t0]
-    i32 = lambda x: torch.tensor(x, dtype=torch.int32, device=DEV)
-    scale = 1.0 / math.sqrt(KV.HD)
-    d_work, d_slot, d_qs = i32(work), i32(list(range(n))), i32(q_start)
-    d_ql, d_past = i32([q for _, q in specs]), i32([p for p, _ in specs])
-    L.check(L.lib().sb200_attn_prefill(
-        L.ptr(qkv), L.ptr(out), L.ptr(pool), L.ptr(pt), max_pages, L.ptr(d_work),
-        len(work) // 2, L.ptr(d_slot), L.ptr(d_qs), L.ptr(d_ql), L.ptr(d_past), hq, hkv, scale,
-        stream()))
-    torch.cuda.synchronize()
-    refs = [attn_ref64(qkv[q_start[i]:q_start[i] + q, :hq * KV.HD].view(q, hq, KV.HD), ks[i],
-                       vs[i], p + 1 + torch.arange(q), hkv) for i, (p, q) in enumerate(specs)]
-    assert_within_bound(out, torch.cat([r for r, _ in refs]), torch.cat([m for _, m in refs]),
-                        f"paged prefill {hq}/{hkv}")
+                        f"decode {hq}/{hkv}")
 
 
 def _dense_case(hq, hkv, specs, prefix_rows, n_layers, layer, seed, q_gain=1.0, t_pad=7):
@@ -327,6 +290,7 @@ def _dense_case(hq, hkv, specs, prefix_rows, n_layers, layer, seed, q_gain=1.0, 
     qkv[:, :hq * KV.HD] *= q_gain
     pre = bf(torch.randn(n_layers, max(prefix_rows, 1), 2 * hkv * KV.HD, device=DEV))
     qt = L.lib().sb200_attn_prefill_q_tile(hq, hkv)
+    assert qt == 128 // (hq // hkv)
     q_start, items, acc = [], [], 0
     for i, (p, q) in enumerate(specs):
         q_start.append(acc)

@@ -12,12 +12,13 @@
 // workspaces sized for max(max_prefill_tokens, max_slots) tokens, a logits
 // chunk, the page table and the per-slot decode state.
 #include <algorithm>
-#include <functional>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/sutro_b200.h"
 #include "common.cuh"
+#include "dev_buf.h"
 #include "kernels.h"
 
 namespace sb {
@@ -172,11 +173,41 @@ __global__ void scatter_logits_kernel(const float* __restrict__ logits,
   for (int i = threadIdx.x; i < vocab / 4; i += blockDim.x) d[i] = src[i];
 }
 
-template <typename T>
-int dmalloc(T** p, size_t n) {
-  SB_CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
-  return 0;
-}
+// The prefill staging buffer: what one prefill step builds on the host, uploaded in one copy.
+// Its sections follow each other in the order of View's fields; offsets count int32 words.
+struct StageLayout {
+  struct View {     // the sections of one buffer, host or device
+    SeqInit* seqs;  // [n_seqs]
+    int32_t* pt;    // [n_seqs][max_pages] page-table rows
+    int32_t* work;  // [n_work][2] {sequence, first query token}: dense prefill attention items
+    int32_t *slot, *q_start, *q_len, *past;  // [n_seqs] each: that attention's sequence arrays
+    int32_t* copy;  // [n_seqs] page to seed with the shared prefix's partial last page, or -1
+  };
+  size_t pt, work, slot, q_start, q_len, past, copy, words;  // offsets, and the total
+
+  StageLayout(size_t n_seqs, size_t n_work, size_t max_pages)
+      : pt(n_seqs * (sizeof(SeqInit) / 4)),
+        work(pt + n_seqs * max_pages),
+        slot(work + 2 * n_work),
+        q_start(slot + n_seqs),
+        q_len(q_start + n_seqs),
+        past(q_len + n_seqs),
+        copy(past + n_seqs),
+        words(copy + n_seqs) {}
+  View at(int32_t* base) const {
+    return {reinterpret_cast<SeqInit*>(base), base + pt,    base + work, base + slot,
+            base + q_start,                   base + q_len, base + past, base + copy};
+  }
+};
+static_assert(sizeof(SeqInit) % 4 == 0, "SeqInit records are staged as int32 words");
+
+// What forward() needs of a prefill step (device pointers into the staging buffer).
+struct PrefillStep {
+  const int32_t* work;  // work items of the dense prefill attention
+  int n_work;
+  const int32_t *q_start, *q_len, *past;  // per sequence
+  bool keep_prefix;  // this pass is the shared prefix's: keep its K/V in prefix_kv
+};
 
 }  // namespace
 
@@ -189,50 +220,37 @@ struct Engine {
   int64_t num_pages = 0;
   size_t layer_stride = 0;  // elements between consecutive layers in the KV pool
 
-  bf16 *x = nullptr, *h = nullptr, *qkv = nullptr, *attn = nullptr, *act = nullptr, *hl = nullptr,
-       *hn = nullptr, *kv_pool = nullptr;
-  float *logits = nullptr, *embed_tmp = nullptr;
-  int32_t *tok_ids = nullptr, *tok_pos = nullptr, *tok_slot = nullptr, *ctx_len = nullptr,
-          *row_slot = nullptr, *last_idx = nullptr, *page_table = nullptr;
-  int32_t *slot_state = nullptr, *slot_ngen = nullptr, *slot_next_tok = nullptr,
-          *slot_pos = nullptr, *slot_done = nullptr, *slot_row = nullptr, *slot_maxnew = nullptr;
-  float* slot_cum_logprob = nullptr;
-  // staging
-  int32_t *h_stage = nullptr, *d_stage = nullptr;
-  size_t stage_cap = 0;  // int32 elements
-  int32_t* h_done = nullptr;
+  DevArray<bf16> x, h, qkv, attn, act, hl, hn, kv_pool;
+  DevArray<float> logits, embed_tmp;
+  DevArray<int32_t> tok_ids, tok_pos, tok_slot, ctx_len, row_slot, last_idx, page_table;
+  DevArray<int32_t> slot_state, slot_ngen, slot_next_tok, slot_pos, slot_done, slot_row,
+      slot_maxnew;
+  DevArray<float> slot_cum_logprob;
+  // Staging: a prefill step's StageLayout, or a decode step's row_slot.  The host buffer is
+  // written only after the stream has been synchronised since its previous copy was enqueued:
+  // every step that copies it is followed by a synchronise (JobRun::retire, or the one after
+  // the shared prefix's pass) before the next step writes it.
+  int32_t* h_stage = nullptr;  // pinned
+  DevArray<int32_t> d_stage;
+  int32_t* h_done = nullptr;  // pinned
   // vocabulary bytes + FSM tables
-  uint8_t* d_tok_bytes = nullptr;
-  int32_t* d_tok_off = nullptr;
-  int32_t* d_fsm_trans = nullptr;
-  uint8_t *d_fsm_accept = nullptr, *d_fsm_final = nullptr;
-  uint32_t* d_mask_bits = nullptr;
-  int32_t *d_tail_off = nullptr, *d_tail_tok = nullptr;  // jump-forward terminal tails
+  DevArray<uint8_t> d_tok_bytes;
+  DevArray<int32_t> d_tok_off, d_fsm_trans;
+  DevArray<uint8_t> d_fsm_accept, d_fsm_final;
+  DevArray<uint32_t> d_mask_bits;
+  DevArray<int32_t> d_tail_off, d_tail_tok;  // jump-forward terminal tails
   int mask_words = 0;
-  size_t fsm_cap_states = 0;
   // job-scoped prompt pieces
-  int32_t *d_prefix = nullptr, *d_suffix = nullptr;
-  int prefix_cap = 0, suffix_cap = 0;
+  DevArray<int32_t> d_prefix, d_suffix;
   // host page allocator
   std::vector<int32_t> free_pages;
   Profiler prof;
-  double gemm_flops = 0, attn_decode_bytes = 0;
+  double gemm_flops = 0;
   int device = 0;
-  bf16* prefix_kv = nullptr;  // [n_layers][prefix_rows][2*hkv*128]: dense K|V of the shared prefix
+  DevArray<bf16> prefix_kv;  // [n_layers][prefix_rows][2*hkv*128]: dense K|V of the shared prefix
   int prefix_rows = 0;
-  bool fill_prefix = false;   // this forward pass is the prefix prefill: keep its K/V
 
   ~Engine() {
-    for (void* p : {(void*)x, (void*)h, (void*)qkv, (void*)attn, (void*)act, (void*)hl, (void*)hn,
-                    (void*)kv_pool, (void*)logits, (void*)embed_tmp, (void*)tok_ids,
-                    (void*)tok_pos, (void*)tok_slot, (void*)ctx_len, (void*)row_slot,
-                    (void*)last_idx, (void*)page_table, (void*)slot_state, (void*)slot_ngen,
-                    (void*)slot_next_tok, (void*)slot_pos, (void*)slot_done, (void*)slot_row,
-                    (void*)slot_maxnew, (void*)slot_cum_logprob, (void*)d_stage, (void*)d_tok_bytes, (void*)d_tok_off,
-                    (void*)d_fsm_trans, (void*)d_fsm_accept, (void*)d_fsm_final,
-                    (void*)d_mask_bits, (void*)d_prefix, (void*)d_suffix, (void*)d_tail_off,
-                    (void*)d_tail_tok, (void*)prefix_kv})
-      cudaFree(p);
     if (h_stage) cudaFreeHost(h_stage);
     if (h_done) cudaFreeHost(h_done);
     if (stream) cudaStreamDestroy(stream);
@@ -248,26 +266,30 @@ struct Engine {
     t_max = std::max(c.max_prefill_tokens, c.max_slots);
     logit_rows = std::min(std::max(c.logit_chunk_rows, 1), std::max(c.max_slots, 1));
     q_tile = attn_prefill_q_tile(c.n_q_heads, c.n_kv_heads);
+    if (q_tile <= 0) {
+      set_last_error("engine_create: GQA group %d is too large", c.n_q_heads / c.n_kv_heads);
+      return -1;
+    }
     num_pages = c.num_pages;
     layer_stride = num_pages * kv_page_elems(c.n_kv_heads);
     SB_CUDA_CHECK(cudaGetDevice(&device));
     SB_CUDA_CHECK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
     const size_t T = t_max, S = c.max_slots + 2;  // +prefix slot, +dummy slot
-    if (dmalloc(&x, T * c.d_model) || dmalloc(&h, T * c.d_model) || dmalloc(&qkv, T * qkv_dim) ||
-        dmalloc(&attn, T * q_dim) || dmalloc(&act, T * c.d_ff) ||
-        dmalloc(&hl, static_cast<size_t>(c.max_slots) * c.d_model) ||
-        dmalloc(&hn, static_cast<size_t>(c.max_slots) * c.d_model) ||
-        dmalloc(&kv_pool, layer_stride * c.n_layers) ||
-        dmalloc(&tok_ids, T) || dmalloc(&tok_pos, T) || dmalloc(&tok_slot, T) ||
-        dmalloc(&ctx_len, S) || dmalloc(&row_slot, S) || dmalloc(&last_idx, S) ||
-        dmalloc(&page_table, S * max_pages) || dmalloc(&slot_state, S) || dmalloc(&slot_ngen, S) ||
-        dmalloc(&slot_next_tok, S) || dmalloc(&slot_pos, S) || dmalloc(&slot_done, S) ||
-        dmalloc(&slot_row, S) || dmalloc(&slot_maxnew, S) || dmalloc(&slot_cum_logprob, S))
+    if (x.alloc(T * c.d_model) || h.alloc(T * c.d_model) || qkv.alloc(T * qkv_dim) ||
+        attn.alloc(T * q_dim) || act.alloc(T * c.d_ff) ||
+        hl.alloc(static_cast<size_t>(c.max_slots) * c.d_model) ||
+        hn.alloc(static_cast<size_t>(c.max_slots) * c.d_model) ||
+        kv_pool.alloc(layer_stride * c.n_layers) ||
+        tok_ids.alloc(T) || tok_pos.alloc(T) || tok_slot.alloc(T) ||
+        ctx_len.alloc(S) || row_slot.alloc(S) || last_idx.alloc(S) ||
+        page_table.alloc(S * max_pages) || slot_state.alloc(S) || slot_ngen.alloc(S) ||
+        slot_next_tok.alloc(S) || slot_pos.alloc(S) || slot_done.alloc(S) ||
+        slot_row.alloc(S) || slot_maxnew.alloc(S) || slot_cum_logprob.alloc(S))
       return -1;
     if (c.embedding_model) {
-      if (dmalloc(&embed_tmp, static_cast<size_t>(c.max_slots) * c.d_model)) return -1;
+      if (embed_tmp.alloc(static_cast<size_t>(c.max_slots) * c.d_model)) return -1;
     } else {
-      if (dmalloc(&logits, static_cast<size_t>(logit_rows) * c.vocab)) return -1;
+      if (logits.alloc(static_cast<size_t>(logit_rows) * c.vocab)) return -1;
     }
     // K/V tiles must hold finite values everywhere (masked P * V must stay 0); the same goes
     // for the k/v columns of the qkv buffer, which the dense prefill attention reads in
@@ -276,10 +298,13 @@ struct Engine {
     SB_CUDA_CHECK(cudaMemsetAsync(qkv, 0, T * qkv_dim * sizeof(bf16), stream));
     SB_CUDA_CHECK(cudaMemsetAsync(page_table, 0, S * max_pages * sizeof(int32_t), stream));
     SB_CUDA_CHECK(cudaMemsetAsync(slot_done, 0, S * sizeof(int32_t), stream));
-    stage_cap = (sizeof(SeqInit) / 4) * S + static_cast<size_t>(S) * max_pages + 2 * (T / 16 + S) +
-                5 * S + 64;
-    SB_CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&h_stage), stage_cap * 4));
-    if (dmalloc(&d_stage, stage_cap)) return -1;
+    // A prefill step has at most max_slots sequences and t_max tokens; a sequence of q_len
+    // tokens has ceil(q_len / q_tile) work items, so the step has at most t_max / q_tile +
+    // max_slots of them.
+    const size_t stage_words =
+        StageLayout(c.max_slots, t_max / q_tile + c.max_slots, max_pages).words;
+    SB_CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&h_stage), stage_words * 4));
+    if (d_stage.alloc(stage_words)) return -1;
     SB_CUDA_CHECK(cudaMallocHost(reinterpret_cast<void**>(&h_done), S * 4));
     free_pages.reserve(num_pages);
     for (int64_t p = num_pages - 1; p >= 0; --p) free_pages.push_back(static_cast<int32_t>(p));
@@ -287,18 +312,19 @@ struct Engine {
     return 0;
   }
 
+  // Every GEMM of the stack and of the LM head: adds its FLOPs to the job's count and launches.
+  int gemm(const void* a, int a_rows, const void* wt, void* d, const void* r, int M, int N, int K,
+           int ldd, int epi, const QkvEpiArgs* qa = nullptr) {
+    gemm_flops += 2.0 * M * N * K;
+    return gemm_bf16_tn(a, a_rows, wt, d, r, M, N, K, ldd, epi, 0, stream, qa);
+  }
+
   // ---- one pass of the transformer stack over T flattened tokens -----------
-  // prefill: attention over (cached prefix | new tokens) per sequence;
-  // decode : one token per sequence against its paged history.
-  int forward(int T, bool prefill, const int32_t* d_work, int n_work,
-              const int32_t* d_seq_q_start, const int32_t* d_seq_q_len, const int32_t* d_seq_past) {
+  // prefill (pf != nullptr): attention over (cached prefix | new tokens) per sequence;
+  // decode (pf == nullptr): one token per sequence against its paged history.
+  int forward(int T, const PrefillStep* pf) {
     const auto& c = cfg;
     const float scale = 1.0f / sqrtf(static_cast<float>(kHeadDim));
-    auto gemm = [&](const void* a, const void* wt, void* d, const void* r, int M, int N, int K,
-                    int ldd, int epi) {
-      gemm_flops += 2.0 * M * N * K;
-      return gemm_bf16_tn(a, t_max, wt, d, r, M, N, K, ldd, epi, 0, stream);
-    };
     SB_K(SB200_KC_EMBED, embed_gather(tok_ids, w.embed, x, T, c.d_model, stream));
     for (int l = 0; l < c.n_layers; ++l) {
       SB_K(SB200_KC_NORM, rmsnorm(x, ln1[l], h, T, c.d_model, c.rms_eps, stream));
@@ -306,33 +332,32 @@ struct Engine {
       // prefill it also leaves K/V in their qkv columns for the dense prefill attention
       QkvEpiArgs qa{tok_pos, tok_slot, page_table, max_pages, kv_layer(l), w.rope_cos,
                     w.rope_sin, qn[l], kn[l], c.n_q_heads, c.n_kv_heads, c.rms_eps,
-                    prefill ? 1 : 0};
-      gemm_flops += 2.0 * T * qkv_dim * c.d_model;
-      SB_K(SB200_KC_GEMM, gemm_bf16_tn(h, t_max, wqkv[l], qkv, nullptr, T, qkv_dim, c.d_model,
-                                       qkv_dim, EPI_QKV_ROPE, 0, stream, &qa));
-      if (prefill && fill_prefix && prefix_kv != nullptr) {
+                    pf ? 1 : 0};
+      SB_K(SB200_KC_GEMM, gemm(h, t_max, wqkv[l], qkv, nullptr, T, qkv_dim, c.d_model, qkv_dim,
+                               EPI_QKV_ROPE, &qa));
+      if (pf && pf->keep_prefix) {
         // the shared prefix's K/V (k|v columns of its rows) go to the dense side buffer
         const size_t cols = 2ull * c.n_kv_heads * kHeadDim;
         SB_CUDA_CHECK(cudaMemcpy2DAsync(prefix_kv + static_cast<size_t>(l) * prefix_rows * cols,
                                         cols * sizeof(bf16), qkv + q_dim, qkv_dim * sizeof(bf16),
                                         cols * sizeof(bf16), T, cudaMemcpyDeviceToDevice, stream));
       }
-      if (prefill) {
+      if (pf) {
         SB_K(SB200_KC_ATTN_PREFILL,
-             attn_prefill_dense(qkv, t_max, attn, prefix_kv, prefix_rows, c.n_layers, l, d_work,
-                                n_work, d_seq_q_start, d_seq_q_len, d_seq_past, c.n_q_heads,
+             attn_prefill_dense(qkv, t_max, attn, prefix_kv, prefix_rows, c.n_layers, l, pf->work,
+                                pf->n_work, pf->q_start, pf->q_len, pf->past, c.n_q_heads,
                                 c.n_kv_heads, scale, stream));
       } else {
         SB_K(SB200_KC_ATTN_DECODE,
              attn_decode(qkv, attn, kv_layer(l), page_table, max_pages, row_slot, ctx_len, T,
                          c.n_q_heads, c.n_kv_heads, scale, stream));
       }
-      SB_K(SB200_KC_GEMM, gemm(attn, wo[l], x, x, T, c.d_model, q_dim, c.d_model,
+      SB_K(SB200_KC_GEMM, gemm(attn, t_max, wo[l], x, x, T, c.d_model, q_dim, c.d_model,
                                EPI_RESIDUAL_BF16));
       SB_K(SB200_KC_NORM, rmsnorm(x, ln2[l], h, T, c.d_model, c.rms_eps, stream));
-      SB_K(SB200_KC_GEMM, gemm(h, wgu[l], act, nullptr, T, 2 * c.d_ff, c.d_model, c.d_ff,
+      SB_K(SB200_KC_GEMM, gemm(h, t_max, wgu[l], act, nullptr, T, 2 * c.d_ff, c.d_model, c.d_ff,
                                EPI_SWIGLU_BF16));
-      SB_K(SB200_KC_GEMM, gemm(act, wd[l], x, x, T, c.d_model, c.d_ff, c.d_model,
+      SB_K(SB200_KC_GEMM, gemm(act, t_max, wd[l], x, x, T, c.d_model, c.d_ff, c.d_model,
                                EPI_RESIDUAL_BF16));
     }
     return 0;
@@ -349,13 +374,12 @@ struct Engine {
       src = hl;
     }
     SB_K(SB200_KC_NORM, rmsnorm(src, w.final_norm, hn, n, c.d_model, c.rms_eps, stream));
+    const bool has_tails = has_fsm && job.fsm_tail_off != nullptr;
     for (int r0 = 0; r0 < n; r0 += logit_rows) {
       const int nr = std::min(logit_rows, n - r0);
-      gemm_flops += 2.0 * nr * c.vocab * c.d_model;
-      SB_K(SB200_KC_GEMM,
-           gemm_bf16_tn(hn + static_cast<size_t>(r0) * c.d_model, c.max_slots - r0, w.lm_head,
-                        logits, nullptr, nr, c.vocab, c.d_model, c.vocab, EPI_STORE_F32, 0,
-                        stream));
+      SB_K(SB200_KC_GEMM, gemm(hn + static_cast<size_t>(r0) * c.d_model, c.max_slots - r0,
+                               w.lm_head, logits, nullptr, nr, c.vocab, c.d_model, c.vocab,
+                               EPI_STORE_F32));
       if (first_decision && job.out_first_logits_dev) {
         scatter_logits_kernel<<<nr, 256, 0, stream>>>(logits, d_row_slot + r0, slot_row,
                                                       job.out_first_logits_dev, c.vocab);
@@ -377,13 +401,14 @@ struct Engine {
       a.out_tokens = job.out_tokens_dev;
       a.out_len = job.out_len_dev;
       a.out_stride = job.max_new_tokens;
-      a.mask_bits = has_fsm ? d_mask_bits : nullptr;
+      a.mask_bits = has_fsm ? d_mask_bits.get() : nullptr;
       a.mask_words = mask_words;
       a.fsm_trans = d_fsm_trans;
       a.fsm_accept = d_fsm_accept;
       a.fsm_final = d_fsm_final;
-      a.fsm_tail_off = has_fsm ? d_tail_off : nullptr;
-      a.fsm_tail_tok = d_tail_tok;
+      // the tail buffers outlive the job that uploaded them: only this job's are passed
+      a.fsm_tail_off = has_tails ? d_tail_off.get() : nullptr;
+      a.fsm_tail_tok = has_tails ? d_tail_tok.get() : nullptr;
       a.tok_bytes = d_tok_bytes;
       a.tok_off = d_tok_off;
       a.eos_id = c.eos_id;
@@ -394,7 +419,7 @@ struct Engine {
       a.seed = job.seed;
       a.seed_per_row = job.seed_per_row;
       a.row_ids = job.row_ids_dev;
-      a.slot_cum_logprob = job.out_cum_logprob_dev ? slot_cum_logprob : nullptr;
+      a.slot_cum_logprob = job.out_cum_logprob_dev ? slot_cum_logprob.get() : nullptr;
       a.out_cum_logprob = job.out_cum_logprob_dev;
       SB_K(SB200_KC_SAMPLE, sample_greedy(a, stream));
     }
@@ -408,28 +433,16 @@ struct Engine {
       return -1;
     }
     mask_words = (cfg.vocab + 31) / 32;
-    if (n > fsm_cap_states) {
-      cudaFree(d_fsm_trans);
-      cudaFree(d_fsm_accept);
-      cudaFree(d_fsm_final);
-      cudaFree(d_mask_bits);
-      d_fsm_trans = nullptr, d_fsm_accept = nullptr, d_fsm_final = nullptr, d_mask_bits = nullptr;
-      fsm_cap_states = 0;
-      if (dmalloc(&d_fsm_trans, n * 256) || dmalloc(&d_fsm_accept, n) || dmalloc(&d_fsm_final, n) ||
-          dmalloc(&d_mask_bits, n * mask_words))
-        return -1;
-      fsm_cap_states = n;
-    }
+    if (d_fsm_trans.reserve(n * 256) || d_fsm_accept.reserve(n) || d_fsm_final.reserve(n) ||
+        d_mask_bits.reserve(n * mask_words))
+      return -1;
     SB_CUDA_CHECK(cudaMemcpyAsync(d_fsm_trans, job.fsm_trans, n * 256 * 4, cudaMemcpyHostToDevice,
                                   stream));
     SB_CUDA_CHECK(cudaMemcpyAsync(d_fsm_accept, job.fsm_accept, n, cudaMemcpyHostToDevice, stream));
     SB_CUDA_CHECK(cudaMemcpyAsync(d_fsm_final, job.fsm_final, n, cudaMemcpyHostToDevice, stream));
-    cudaFree(d_tail_off);
-    cudaFree(d_tail_tok);
-    d_tail_off = nullptr, d_tail_tok = nullptr;
     if (job.fsm_tail_off != nullptr) {
       const size_t nt = job.fsm_tail_off[n];
-      if (dmalloc(&d_tail_off, n + 1) || dmalloc(&d_tail_tok, nt > 0 ? nt : 1)) return -1;
+      if (d_tail_off.reserve(n + 1) || d_tail_tok.reserve(nt > 0 ? nt : 1)) return -1;
       SB_CUDA_CHECK(cudaMemcpyAsync(d_tail_off, job.fsm_tail_off, (n + 1) * 4, cudaMemcpyHostToDevice,
                                     stream));
       if (nt)
@@ -443,72 +456,48 @@ struct Engine {
   int run(const sb200_job& job, sb200_job_stats* stats);
 };
 
-// ---------------------------------------------------------------------------
-// the scheduling loop
-// ---------------------------------------------------------------------------
-int Engine::run(const sb200_job& job, sb200_job_stats* stats) {
-  const auto& c = cfg;
-  const int64_t N = job.n_rows;
-  SB_CUDA_CHECK(cudaSetDevice(device));
-  prof.reset(job.profile != 0, stream);
-  gemm_flops = 0;
-  attn_decode_bytes = 0;
-  const bool embed_mode = c.embedding_model != 0;
-  const bool has_fsm = !embed_mode && job.fsm_states > 0;
-  const int max_new = embed_mode ? 0 : job.max_new_tokens;
-  if (N <= 0) return 0;
-  if (!embed_mode && max_new <= 0) {
+namespace {
+
+// The parameters of one job, checked before anything is uploaded.
+struct JobSpec {
+  bool embed_mode = false, has_fsm = false;
+  int max_new = 0, n_prefix = 0, n_suffix = 0, n_forced = 0;
+  int prefix_cached = 0;           // prefix tokens whose K/V are computed once for every row
+  std::vector<int32_t> n_row_tok;  // prompt tokens of each row, after truncation
+  int64_t n_truncated = 0;
+};
+
+int validate_job(const sb200_engine_config& c, const sb200_job& job, JobSpec& s) {
+  s.embed_mode = c.embedding_model != 0;
+  s.has_fsm = !s.embed_mode && job.fsm_states > 0;
+  s.max_new = s.embed_mode ? 0 : job.max_new_tokens;
+  if (!s.embed_mode && s.max_new <= 0) {
     set_last_error("engine: max_new_tokens must be positive");
     return -1;
   }
-  if (embed_mode ? job.out_embed_dev == nullptr
-                 : (job.out_tokens_dev == nullptr || job.out_len_dev == nullptr)) {
+  if (s.embed_mode ? job.out_embed_dev == nullptr
+                   : (job.out_tokens_dev == nullptr || job.out_len_dev == nullptr)) {
     set_last_error("engine: output buffers missing");
     return -1;
   }
-  const int n_prefix = job.n_prefix, n_suffix = job.n_suffix;
-  const int n_forced = (has_fsm && job.n_forced_prefix > 0) ? job.n_forced_prefix : 0;
-  if (n_forced > n_suffix || (n_forced > 0 && n_forced >= max_new)) {
+  s.n_prefix = job.n_prefix;
+  s.n_suffix = job.n_suffix;
+  s.n_forced = (s.has_fsm && job.n_forced_prefix > 0) ? job.n_forced_prefix : 0;
+  if (s.n_forced > s.n_suffix || (s.n_forced > 0 && s.n_forced >= s.max_new)) {
     set_last_error("engine: forced output prefix (%d tokens) does not fit suffix/max_new_tokens",
-                   n_forced);
+                   s.n_forced);
     return -1;
   }
-  const int ctx_budget = c.max_position - max_new;  // prompt tokens that fit
-  if (n_prefix + n_suffix + 1 > ctx_budget) {
+  const int ctx_budget = c.max_position - s.max_new;  // prompt tokens that fit
+  if (s.n_prefix + s.n_suffix + 1 > ctx_budget) {
     set_last_error("engine: system prompt + template (%d tokens) leave no room in the %d-token "
-                   "context window", n_prefix + n_suffix, c.max_position);
+                   "context window", s.n_prefix + s.n_suffix, c.max_position);
     return -1;
   }
-  // prompt pieces -> device
-  if (n_prefix > prefix_cap) {
-    cudaFree(d_prefix);
-    d_prefix = nullptr;
-    if (dmalloc(&d_prefix, static_cast<size_t>(n_prefix))) return -1;
-    prefix_cap = n_prefix;
-  }
-  if (n_suffix > suffix_cap) {
-    cudaFree(d_suffix);
-    d_suffix = nullptr;
-    if (dmalloc(&d_suffix, static_cast<size_t>(n_suffix))) return -1;
-    suffix_cap = n_suffix;
-  }
-  if (n_prefix)
-    SB_CUDA_CHECK(cudaMemcpyAsync(d_prefix, job.prefix_tokens, n_prefix * 4ull,
-                                  cudaMemcpyHostToDevice, stream));
-  if (n_suffix)
-    SB_CUDA_CHECK(cudaMemcpyAsync(d_suffix, job.suffix_tokens, n_suffix * 4ull,
-                                  cudaMemcpyHostToDevice, stream));
-  if (has_fsm && upload_fsm(job)) return -1;
-  if (!embed_mode)
-    SB_CUDA_CHECK(cudaMemsetAsync(job.out_len_dev, 0, N * sizeof(int32_t), stream));
-
-  // per-row prompt lengths (host)
-  const int64_t* roff = job.row_tok_off;
-  std::vector<int32_t> n_row_tok(N);
-  int64_t n_truncated = 0;
-  for (int64_t r = 0; r < N; ++r) {
-    int64_t n = roff[r + 1] - roff[r];
-    const int64_t room = ctx_budget - n_prefix - n_suffix;
+  const int64_t room = ctx_budget - s.n_prefix - s.n_suffix;
+  s.n_row_tok.resize(job.n_rows);
+  for (int64_t r = 0; r < job.n_rows; ++r) {
+    int64_t n = job.row_tok_off[r + 1] - job.row_tok_off[r];
     if (n > room) {
       if (!job.truncate_rows) {
         set_last_error("engine: row %lld has %lld tokens but only %lld fit the context window "
@@ -516,213 +505,230 @@ int Engine::run(const sb200_job& job, sb200_job_stats* stats) {
         return -1;
       }
       n = room;
-      ++n_truncated;
+      ++s.n_truncated;
     }
-    n_row_tok[r] = static_cast<int32_t>(n);
+    s.n_row_tok[r] = static_cast<int32_t>(n);
+  }
+  s.prefix_cached = (job.share_prefix && s.n_prefix >= kPageTokens) ? s.n_prefix : 0;
+  if (s.prefix_cached > c.max_prefill_tokens) {
+    set_last_error("engine: shared prefix (%d tokens) exceeds max_prefill_tokens", s.prefix_cached);
+    return -1;
+  }
+  return 0;
+}
+
+// One sb200_engine_run call: the checked job, the host bookkeeping of its slots and pages, its
+// counters, and one method per scheduling step.  Destroying it hands the job's pages back to the
+// engine's pool, however the run ends.
+struct JobRun {
+  Engine& e;
+  const sb200_job& job;
+  const JobSpec p;
+  const int S;  // decode slots; slot S (page-table row S) holds the shared prefix
+  std::vector<std::vector<int32_t>> slot_pages;  // [S + 1] pages owned by each slot
+  std::vector<int32_t> free_slots;
+  std::vector<int32_t> active;    // slots in the decode batch
+  std::vector<int32_t> slot_ctx;  // host mirror: position of the next fed token
+  std::vector<SeqInit> batch;     // the sequences of the next prefill step
+  int prefix_tail_page = -1;      // physical page holding the partial tail of the shared prefix
+  int64_t next_row = 0, rows_done = 0, in_tokens = 0, prefill_tokens = 0, decode_tokens = 0;
+  int64_t steps_prefill = 0, steps_decode = 0;
+  double attn_decode_bytes = 0;
+
+  JobRun(Engine& engine, const sb200_job& j, JobSpec spec)
+      : e(engine), job(j), p(std::move(spec)), S(engine.cfg.max_slots), slot_pages(S + 1),
+        slot_ctx(S, 0) {
+    for (int s = S - 1; s >= 0; --s) free_slots.push_back(s);
+  }
+  ~JobRun() {
+    for (const auto& v : slot_pages) e.free_pages.insert(e.free_pages.end(), v.begin(), v.end());
   }
 
-  // staging layout (int32 units)
-  const int S = c.max_slots;
-  const int prefix_slot = S;  // page-table row S holds the shared prefix
-  SeqInit* h_seqs = reinterpret_cast<SeqInit*>(h_stage);
-  const size_t seq_words = (sizeof(SeqInit) / 4) * (S + 2);
-  int32_t* h_pt = h_stage + seq_words;
-  int32_t* h_work = h_pt + static_cast<size_t>(S + 2) * max_pages;
-  int32_t* h_misc = h_work + 2 * (t_max / 16 + S + 2);  // seq_slot|q_start|q_len|past : 4*(S+2)
-  int32_t* h_copy = h_misc + 4 * (S + 2);               // first own page to seed, or -1
-  const SeqInit* d_seqs = reinterpret_cast<const SeqInit*>(d_stage);
-  const int32_t* d_pt = d_stage + seq_words;
-  const int32_t* d_work = d_pt + static_cast<size_t>(S + 2) * max_pages;
-  const int32_t* d_misc = d_work + 2 * (t_max / 16 + S + 2);
-  const int32_t* d_copy = d_misc + 4 * (S + 2);
-  int prefix_tail_page = -1;  // physical page holding the partial tail of the shared prefix
-
-  std::vector<int32_t> prefix_pages;
-  std::vector<std::vector<int32_t>> slot_pages(S);
-  std::vector<int32_t> free_slots;
-  for (int s = S - 1; s >= 0; --s) free_slots.push_back(s);
-  std::vector<int32_t> active;  // slots in the decode batch
-  std::vector<int32_t> slot_ctx(S, 0);  // host mirror: position of the next fed token
-
-  auto release_all = [&]() {
-    for (auto& v : slot_pages) {
-      for (int32_t p : v) free_pages.push_back(p);
-      v.clear();
-    }
-    for (int32_t p : prefix_pages) free_pages.push_back(p);
-    prefix_pages.clear();
-  };
-
-  // every exit path of run() (early error returns included) hands the pages back to the
-  // engine-lifetime pool; release_all is idempotent
-  struct ReleaseGuard {
-    std::function<void()> f;
-    ~ReleaseGuard() { f(); }
-  } release_guard{release_all};
-
-  // Launch one prefill step for seqs h_seqs[0..n) (page rows in h_pt), T tokens total.
-  auto run_prefill = [&](int n, int T, bool sample) -> int {
-    int n_work = 0;
-    for (int i = 0; i < n; ++i) {
-      h_misc[i] = h_seqs[i].slot;
-      h_misc[(S + 2) + i] = h_seqs[i].q_start;
-      h_misc[2 * (S + 2) + i] = h_seqs[i].q_len;
-      h_misc[3 * (S + 2) + i] = h_seqs[i].past;
-      for (int t0 = 0; t0 < h_seqs[i].q_len; t0 += q_tile) {
-        h_work[2 * n_work] = i;
-        h_work[2 * n_work + 1] = t0;
-        ++n_work;
-      }
-    }
-    SB_CUDA_CHECK(cudaMemcpyAsync(d_stage, h_stage, stage_cap * 4, cudaMemcpyHostToDevice, stream));
-    prof.launches[SB200_KC_OTHER] += 2;
-    init_slots_kernel<<<n, 128, 0, stream>>>(d_seqs, d_pt, max_pages, page_table, slot_state,
-                                             slot_ngen, slot_pos, slot_done, slot_row, slot_maxnew,
-                                             slot_next_tok, d_suffix + (n_suffix - n_forced),
-                                             n_forced, embed_mode ? nullptr : job.out_tokens_dev,
-                                             embed_mode ? nullptr : job.out_len_dev,
-                                             job.max_new_tokens, slot_cum_logprob);
-    prefill_prepare_kernel<<<n, 128, 0, stream>>>(d_seqs, d_prefix, n_prefix, d_suffix, n_suffix,
-                                                  job.row_tokens_dev, job.row_tok_off_dev, tok_ids,
-                                                  tok_pos, tok_slot, last_idx);
-    if (prefix_tail_page >= 0 && sample) {
-      ++prof.launches[SB200_KC_OTHER];
-      copy_prefix_page_kernel<<<dim3(n, c.n_layers), 256, 0, stream>>>(
-          kv_pool, layer_stride, kv_page_elems(c.n_kv_heads),
-          prefix_tail_page, d_copy);
-    }
-    SB_CUDA_CHECK(cudaGetLastError());
-    if (forward(T, true, d_work, n_work, d_misc + (S + 2), d_misc + 2 * (S + 2),
-                d_misc + 3 * (S + 2)))
-      return -1;
-    if (!sample) return 0;
-    if (embed_mode) {
-      if (gather_rows(last_idx, x, hl, n, c.d_model, stream)) return -1;
-      if (rmsnorm(hl, w.final_norm, hn, n, c.d_model, c.rms_eps, stream)) return -1;
-      if (l2_normalize_rows(hn, embed_tmp, n, c.d_model, stream)) return -1;
-      scatter_embed_kernel<<<n, 128, 0, stream>>>(embed_tmp, d_seqs, job.out_embed_dev, c.d_model);
-      SB_CUDA_CHECK(cudaGetLastError());
-      return 0;
-    }
-    return head_and_sample(n, last_idx, d_misc /* seq_slot */, job, has_fsm, true);
-  };
-
-  // ---- shared prefix: compute its KV once, every row's page table points at it ----
-  // The whole prefix is computed once; full pages are shared through the page tables and
-  // the partially filled last page is copied into each row's first own page.
-  const int prefix_cached = (job.share_prefix && n_prefix >= kPageTokens) ? n_prefix : 0;
-  if (prefix_cached > 0) {
-    if (prefix_cached > c.max_prefill_tokens) {
-      set_last_error("engine: shared prefix (%d tokens) exceeds max_prefill_tokens", prefix_cached);
-      return -1;
-    }
-    const int np = (prefix_cached + kPageTokens - 1) / kPageTokens;
-    if (static_cast<int64_t>(free_pages.size()) < np) {
+  // The shared prefix is prefilled once: its full pages are shared through the page tables,
+  // its partially filled last page is copied into each row's first own page.
+  int cache_prefix() {
+    const int n = p.prefix_cached;
+    if (n == 0) return 0;
+    const int np = (n + kPageTokens - 1) / kPageTokens;
+    if (static_cast<int64_t>(e.free_pages.size()) < np) {
       set_last_error("engine: KV pool too small for the shared prefix");
       return -1;
     }
+    std::vector<int32_t>& pages = slot_pages[S];
     for (int i = 0; i < np; ++i) {
-      prefix_pages.push_back(free_pages.back());
-      free_pages.pop_back();
+      pages.push_back(e.free_pages.back());
+      e.free_pages.pop_back();
     }
-    h_seqs[0] = SeqInit{prefix_slot, -1, 0, prefix_cached, 0, 0, 1, -1};
-    std::fill(h_pt, h_pt + max_pages, 0);
-    std::copy(prefix_pages.begin(), prefix_pages.end(), h_pt);
-    if (prefix_cached > prefix_rows) {
-      cudaFree(prefix_kv);
-      prefix_kv = nullptr;
-      prefix_rows = 0;
-      const size_t n = static_cast<size_t>(c.n_layers) * prefix_cached * 2 * c.n_kv_heads * kHeadDim;
-      if (dmalloc(&prefix_kv, n)) {
-        release_all();
-        return -1;
-      }
-      prefix_rows = prefix_cached;
-      cudaMemsetAsync(prefix_kv, 0, n * sizeof(bf16), stream);
+    if (n > e.prefix_rows) {
+      const size_t elems =
+          static_cast<size_t>(e.cfg.n_layers) * n * 2 * e.cfg.n_kv_heads * kHeadDim;
+      e.prefix_rows = 0;
+      if (e.prefix_kv.alloc(elems)) return -1;
+      e.prefix_rows = n;
+      cudaMemsetAsync(e.prefix_kv, 0, elems * sizeof(bf16), e.stream);
     }
-    fill_prefix = true;
-    const int prc = run_prefill(1, prefix_cached, false);
-    fill_prefix = false;
-    if (prc) {
-      release_all();
-      return -1;
-    }
-    if (prefix_cached % kPageTokens != 0) prefix_tail_page = prefix_pages.back();
-    SB_CUDA_CHECK(cudaStreamSynchronize(stream));
+    batch.assign(1, SeqInit{S, -1, 0, n, 0, 0, 1, -1});
+    if (prefill(n, true)) return -1;
+    if (n % kPageTokens != 0) prefix_tail_page = pages.back();
+    prefill_tokens = n;
+    SB_CUDA_CHECK(cudaStreamSynchronize(e.stream));
+    return 0;
   }
 
-  int64_t next_row = 0, rows_done = 0, in_tokens = 0, steps_prefill = 0, steps_decode = 0;
-  int64_t decode_tokens = 0, prefill_tokens = prefix_cached;
-  int rc = 0;
-
-  auto admit = [&]() -> int {  // returns number of rows admitted, <0 on error
-    int n = 0, T = 0;
-    while (next_row < N && !free_slots.empty() && n < S) {
+  // Takes rows in order while a slot, the prefill budget and the KV pool allow, reserves each
+  // row's pages up front and runs their prefill step.  Returns the rows admitted, or -1.
+  int admit() {
+    const auto& c = e.cfg;
+    batch.clear();
+    int T = 0;
+    while (next_row < job.n_rows && !free_slots.empty() && static_cast<int>(batch.size()) < S) {
       const int64_t r = next_row;
-      const int P = n_prefix + n_row_tok[r] + n_suffix;
+      const int P = p.n_prefix + p.n_row_tok[r] + p.n_suffix;
       if (P <= 0) {
         set_last_error("engine: row %lld renders to an empty prompt", (long long)r);
         return -1;
       }
-      int past = std::min(prefix_cached, P - 1);
-      if (past < prefix_cached) past = (past / kPageTokens) * kPageTokens;  // prompt ends inside the prefix
+      int past = std::min(p.prefix_cached, P - 1);
+      // the prompt ends inside the prefix
+      if (past < p.prefix_cached) past = (past / kPageTokens) * kPageTokens;
       const int q_len = P - past;
       if (T + q_len > c.max_prefill_tokens) {
-        if (n == 0) {
+        if (batch.empty()) {
           set_last_error("engine: row %lld needs %d prefill tokens > max_prefill_tokens=%d",
                          (long long)r, q_len, c.max_prefill_tokens);
           return -1;
         }
         break;
       }
-      const int total_pages = (P + max_new + kPageTokens - 1) / kPageTokens;
+      const int total_pages = (P + p.max_new + kPageTokens - 1) / kPageTokens;
       const int own = total_pages - past / kPageTokens;
-      if (static_cast<int64_t>(free_pages.size()) < own) {
-        if (n == 0 && active.empty()) {
+      if (static_cast<int64_t>(e.free_pages.size()) < own) {
+        if (batch.empty() && active.empty()) {
           set_last_error("engine: KV pool (%lld pages) cannot hold one row of %d tokens",
-                         (long long)num_pages, P + max_new);
+                         (long long)e.num_pages, P + p.max_new);
           return -1;
         }
         break;
       }
       const int slot = free_slots.back();
       free_slots.pop_back();
-      int32_t* pt = h_pt + static_cast<size_t>(n) * max_pages;
-      std::fill(pt, pt + max_pages, 0);
-      for (int i = 0; i < past / kPageTokens; ++i) pt[i] = prefix_pages[i];
-      auto& mine = slot_pages[slot];
-      h_copy[n] = -1;
       for (int i = 0; i < own; ++i) {
-        mine.push_back(free_pages.back());
-        pt[past / kPageTokens + i] = free_pages.back();
-        free_pages.pop_back();
+        slot_pages[slot].push_back(e.free_pages.back());
+        e.free_pages.pop_back();
       }
-      // positions [16*(past/16), past) of the first own page hold prefix tokens: seed them
-      if (past % kPageTokens != 0) h_copy[n] = pt[past / kPageTokens];
-      h_seqs[n] = SeqInit{slot, static_cast<int32_t>(r), T, q_len, past, n_row_tok[r], max_new,
-                          has_fsm ? job.fsm_start : -1};
+      batch.push_back(SeqInit{slot, static_cast<int32_t>(r), T, q_len, past, p.n_row_tok[r],
+                              p.max_new, p.has_fsm ? job.fsm_start : -1});
       slot_ctx[slot] = P;
       T += q_len;
       in_tokens += P;
-      ++n;
       ++next_row;
     }
-    if (n == 0) return 0;
-    if (run_prefill(n, T, true)) return -1;
+    if (batch.empty()) return 0;
+    if (prefill(T, false)) return -1;
     prefill_tokens += T;
     ++steps_prefill;
-    for (int i = 0; i < n; ++i) active.push_back(h_seqs[i].slot);
-    return n;
-  };
+    for (const SeqInit& s : batch) active.push_back(s.slot);
+    return static_cast<int>(batch.size());
+  }
 
-  auto retire = [&]() -> int {  // reads the done flags, frees finished slots
-    SB_CUDA_CHECK(cudaMemcpyAsync(h_done, slot_done, (S + 2) * 4ull, cudaMemcpyDeviceToHost, stream));
-    SB_CUDA_CHECK(cudaStreamSynchronize(stream));
+  // One prefill step over the sequences in `batch`, T new tokens in all: stages and uploads
+  // them, installs their page-table rows and decode state, and runs the stack; then, except in
+  // the shared prefix's own pass, the head: each row's first token, or its embedding.
+  int prefill(int T, bool prefix_pass) {
+    const auto& c = e.cfg;
+    const int n = static_cast<int>(batch.size());
+    int n_work = 0;
+    for (const SeqInit& s : batch) n_work += (s.q_len + e.q_tile - 1) / e.q_tile;
+    const StageLayout L(n, n_work, e.max_pages);
+    const StageLayout::View h = L.at(e.h_stage), d = L.at(e.d_stage);
+    for (int i = 0, wi = 0; i < n; ++i) {
+      const SeqInit& s = batch[i];
+      const std::vector<int32_t>& own = slot_pages[s.slot];
+      const int shared = s.past / kPageTokens;  // full prefix pages before the first own page
+      int32_t* pt = h.pt + static_cast<size_t>(i) * e.max_pages;
+      std::fill(pt, pt + e.max_pages, 0);
+      std::copy(slot_pages[S].begin(), slot_pages[S].begin() + shared, pt);
+      std::copy(own.begin(), own.end(), pt + shared);
+      h.seqs[i] = s;
+      h.slot[i] = s.slot;
+      h.q_start[i] = s.q_start;
+      h.q_len[i] = s.q_len;
+      h.past[i] = s.past;
+      // positions [16*(past/16), past) of the first own page hold prefix tokens: seed them
+      h.copy[i] = s.past % kPageTokens != 0 ? own[0] : -1;
+      for (int t0 = 0; t0 < s.q_len; t0 += e.q_tile, ++wi) {
+        h.work[2 * wi] = i;
+        h.work[2 * wi + 1] = t0;
+      }
+    }
+    SB_CUDA_CHECK(cudaMemcpyAsync(e.d_stage, e.h_stage, L.words * 4, cudaMemcpyHostToDevice,
+                                  e.stream));
+    e.prof.launches[SB200_KC_OTHER] += 2;
+    init_slots_kernel<<<n, 128, 0, e.stream>>>(
+        d.seqs, d.pt, e.max_pages, e.page_table, e.slot_state, e.slot_ngen, e.slot_pos,
+        e.slot_done, e.slot_row, e.slot_maxnew, e.slot_next_tok,
+        e.d_suffix + (p.n_suffix - p.n_forced), p.n_forced,
+        p.embed_mode ? nullptr : job.out_tokens_dev, p.embed_mode ? nullptr : job.out_len_dev,
+        job.max_new_tokens, e.slot_cum_logprob);
+    prefill_prepare_kernel<<<n, 128, 0, e.stream>>>(d.seqs, e.d_prefix, p.n_prefix, e.d_suffix,
+                                                    p.n_suffix, job.row_tokens_dev,
+                                                    job.row_tok_off_dev, e.tok_ids, e.tok_pos,
+                                                    e.tok_slot, e.last_idx);
+    if (prefix_tail_page >= 0) {
+      ++e.prof.launches[SB200_KC_OTHER];
+      copy_prefix_page_kernel<<<dim3(n, c.n_layers), 256, 0, e.stream>>>(
+          e.kv_pool, e.layer_stride, kv_page_elems(c.n_kv_heads), prefix_tail_page, d.copy);
+    }
+    SB_CUDA_CHECK(cudaGetLastError());
+    const PrefillStep step{d.work, n_work, d.q_start, d.q_len, d.past, prefix_pass};
+    if (e.forward(T, &step)) return -1;
+    if (prefix_pass) return 0;
+    if (p.embed_mode) {
+      if (gather_rows(e.last_idx, e.x, e.hl, n, c.d_model, e.stream)) return -1;
+      if (rmsnorm(e.hl, e.w.final_norm, e.hn, n, c.d_model, c.rms_eps, e.stream)) return -1;
+      if (l2_normalize_rows(e.hn, e.embed_tmp, n, c.d_model, e.stream)) return -1;
+      scatter_embed_kernel<<<n, 128, 0, e.stream>>>(e.embed_tmp, d.seqs, job.out_embed_dev,
+                                                    c.d_model);
+      SB_CUDA_CHECK(cudaGetLastError());
+      return 0;
+    }
+    return e.head_and_sample(n, e.last_idx, d.slot, job, p.has_fsm, true);
+  }
+
+  // One decode step: one token for every slot in the decode batch.
+  int decode_step() {
+    const auto& c = e.cfg;
+    const int B = static_cast<int>(active.size());
+    std::copy(active.begin(), active.end(), e.h_stage);
+    SB_CUDA_CHECK(cudaMemcpyAsync(e.row_slot, e.h_stage, B * 4ull, cudaMemcpyHostToDevice,
+                                  e.stream));
+    e.prof.begin(SB200_KC_OTHER);
+    const int prc = prepare_decode(e.row_slot, e.slot_next_tok, e.slot_pos, e.tok_ids, e.tok_pos,
+                                   e.tok_slot, e.ctx_len, B, e.stream);
+    e.prof.end();
+    if (prc || e.forward(B, nullptr) || e.head_and_sample(B, nullptr, e.row_slot, job, p.has_fsm))
+      return -1;
+    decode_tokens += B;
+    ++steps_decode;
+    int64_t ctx_sum = 0;
+    for (int s : active) ctx_sum += ++slot_ctx[s];
+    attn_decode_bytes +=
+        static_cast<double>(ctx_sum) * c.n_layers * c.n_kv_heads * 2.0 * kHeadDim * 2.0;
+    return 0;
+  }
+
+  // Waits for the stream, then frees the slots and pages of finished rows: those whose done
+  // flag is set, or every admitted row of an embedding model (its prefill finished it).
+  int retire() {
+    if (!p.embed_mode)
+      SB_CUDA_CHECK(cudaMemcpyAsync(e.h_done, e.slot_done, (S + 2) * 4ull, cudaMemcpyDeviceToHost,
+                                    e.stream));
+    SB_CUDA_CHECK(cudaStreamSynchronize(e.stream));
     size_t k = 0;
     for (size_t i = 0; i < active.size(); ++i) {
       const int s = active[i];
-      if (h_done[s]) {
-        for (int32_t p : slot_pages[s]) free_pages.push_back(p);
+      if (p.embed_mode || e.h_done[s]) {
+        e.free_pages.insert(e.free_pages.end(), slot_pages[s].begin(), slot_pages[s].end());
         slot_pages[s].clear();
         free_slots.push_back(s);
         ++rows_done;
@@ -732,94 +738,86 @@ int Engine::run(const sb200_job& job, sb200_job_stats* stats) {
     }
     active.resize(k);
     return 0;
-  };
+  }
 
-  const int min_admit = std::max(1, c.min_admit_rows);
-  while (rows_done < N) {
+  void fill_stats(sb200_job_stats* st) const {
+    for (int i = 0; i < SB200_KC_COUNT; ++i) {
+      st->kernel_ms[i] = e.prof.ms[i];
+      st->kernel_launches[i] = e.prof.launches[i];
+    }
+    st->gemm_flops = e.gemm_flops;
+    st->attn_decode_bytes = attn_decode_bytes;
+    st->rows_done = rows_done;
+    st->input_tokens = in_tokens;
+    st->prefill_tokens = prefill_tokens;
+    st->decode_tokens = decode_tokens;
+    st->prefill_steps = steps_prefill;
+    st->decode_steps = steps_decode;
+    st->rows_truncated = p.n_truncated;
+    st->prefix_cached_tokens = p.prefix_cached;
+  }
+};
+
+}  // namespace
+
+// ---------------------------------------------------------------------------
+// the scheduling loop
+// ---------------------------------------------------------------------------
+int Engine::run(const sb200_job& job, sb200_job_stats* stats) {
+  const int64_t N = job.n_rows;
+  SB_CUDA_CHECK(cudaSetDevice(device));
+  prof.reset(job.profile != 0, stream);
+  gemm_flops = 0;
+  if (N <= 0) return 0;
+  JobSpec spec;
+  if (validate_job(cfg, job, spec)) return -1;
+  // prompt pieces and FSM -> device
+  if (d_prefix.reserve(spec.n_prefix) || d_suffix.reserve(spec.n_suffix)) return -1;
+  if (spec.n_prefix)
+    SB_CUDA_CHECK(cudaMemcpyAsync(d_prefix, job.prefix_tokens, spec.n_prefix * 4ull,
+                                  cudaMemcpyHostToDevice, stream));
+  if (spec.n_suffix)
+    SB_CUDA_CHECK(cudaMemcpyAsync(d_suffix, job.suffix_tokens, spec.n_suffix * 4ull,
+                                  cudaMemcpyHostToDevice, stream));
+  if (spec.has_fsm && upload_fsm(job)) return -1;
+  if (!spec.embed_mode)
+    SB_CUDA_CHECK(cudaMemsetAsync(job.out_len_dev, 0, N * sizeof(int32_t), stream));
+
+  JobRun j(*this, job, std::move(spec));
+  if (j.cache_prefix()) return -1;
+  const int min_admit = std::max(1, cfg.min_admit_rows);
+  int rc = 0;
+  while (rc == 0 && j.rows_done < N) {
     // ---- admission: refill free slots with new rows (their prefill) ----
-    const bool can_admit = next_row < N && !free_slots.empty();
-    if (can_admit && (active.empty() || static_cast<int>(free_slots.size()) >= min_admit ||
-                      N - next_row <= static_cast<int64_t>(free_slots.size()))) {
-      const int n = admit();
+    const int64_t n_free = static_cast<int64_t>(j.free_slots.size());
+    if (j.next_row < N && n_free > 0 &&
+        (j.active.empty() || n_free >= min_admit || N - j.next_row <= n_free)) {
+      const int n = j.admit();
       if (n < 0) {
         rc = -1;
         break;
       }
-      if (embed_mode) {
-        // prefill-only: rows are complete, recycle their slots right away
-        SB_CUDA_CHECK(cudaStreamSynchronize(stream));
-        for (int s : active) {
-          for (int32_t p : slot_pages[s]) free_pages.push_back(p);
-          slot_pages[s].clear();
-          free_slots.push_back(s);
-          ++rows_done;
-        }
-        active.clear();
-        if (job.progress) job.progress(rows_done, in_tokens, 0, job.progress_user);
-        continue;
-      }
       if (n > 0) {
-        if (retire()) {
-          rc = -1;
-          break;
-        }
-        if (job.progress) job.progress(rows_done, in_tokens, decode_tokens, job.progress_user);
+        rc = j.retire();
+        if (rc == 0 && job.progress)
+          job.progress(j.rows_done, j.in_tokens, j.decode_tokens, job.progress_user);
         continue;  // try to admit more before decoding
       }
     }
-    if (active.empty()) {
-      if (next_row >= N) break;
+    if (j.active.empty()) {
+      if (j.next_row >= N) break;
       set_last_error("engine: scheduler stalled (no active rows, none admissible)");
       rc = -1;
       break;
     }
     // ---- one decode step over all active rows ----
-    const int B = static_cast<int>(active.size());
-    std::copy(active.begin(), active.end(), h_misc);
-    SB_CUDA_CHECK(cudaMemcpyAsync(row_slot, h_misc, B * 4ull, cudaMemcpyHostToDevice, stream));
-    prof.begin(SB200_KC_OTHER);
-    const int prc = prepare_decode(row_slot, slot_next_tok, slot_pos, tok_ids, tok_pos, tok_slot,
-                                   ctx_len, B, stream);
-    prof.end();
-    if (prc || forward(B, false, nullptr, 0, nullptr, nullptr, nullptr) ||
-        head_and_sample(B, nullptr, row_slot, job, has_fsm)) {
-      rc = -1;
-      break;
-    }
-    decode_tokens += B;
-    ++steps_decode;
-    {
-      int64_t ctx_sum = 0;
-      for (int s : active) ctx_sum += ++slot_ctx[s];
-      attn_decode_bytes += static_cast<double>(ctx_sum) * c.n_layers * c.n_kv_heads * 2.0 *
-                           kHeadDim * 2.0;
-    }
-    if (retire()) {
-      rc = -1;
-      break;
-    }
-    if (job.progress && (steps_decode % 8 == 0 || rows_done == N))
-      job.progress(rows_done, in_tokens, decode_tokens, job.progress_user);
+    rc = (j.decode_step() || j.retire()) ? -1 : 0;
+    if (rc == 0 && job.progress && (j.steps_decode % 8 == 0 || j.rows_done == N))
+      job.progress(j.rows_done, j.in_tokens, j.decode_tokens, job.progress_user);
   }
   cudaStreamSynchronize(stream);
-  release_all();
   prof.resolve();
-  if (stats) {
-    for (int i = 0; i < SB200_KC_COUNT; ++i) {
-      stats->kernel_ms[i] = prof.ms[i];
-      stats->kernel_launches[i] = prof.launches[i];
-    }
-    stats->gemm_flops = gemm_flops;
-    stats->attn_decode_bytes = attn_decode_bytes;
-    stats->rows_done = rows_done;
-    stats->input_tokens = in_tokens;
-    stats->prefill_tokens = prefill_tokens;
-    stats->decode_tokens = decode_tokens;
-    stats->prefill_steps = steps_prefill;
-    stats->decode_steps = steps_decode;
-    stats->rows_truncated = n_truncated;
-    stats->prefix_cached_tokens = prefix_cached;
-  }
+  if (stats) j.fill_stats(stats);
   if (rc == 0) {
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {
@@ -890,12 +888,8 @@ int sb200_engine_set_vocab(void* engine, const uint8_t* tok_bytes, const int32_t
   auto* e = static_cast<Engine*>(engine);
   SB_CUDA_CHECK(cudaSetDevice(e->device));
   const int V = e->cfg.vocab;
-  cudaFree(e->d_tok_bytes);
-  cudaFree(e->d_tok_off);
-  e->d_tok_bytes = nullptr, e->d_tok_off = nullptr;
   const size_t nb = tok_off[V] > 0 ? tok_off[V] : 1;
-  SB_CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&e->d_tok_bytes), nb));
-  SB_CUDA_CHECK(cudaMalloc(reinterpret_cast<void**>(&e->d_tok_off), (V + 1) * 4ull));
+  if (e->d_tok_bytes.alloc(nb) || e->d_tok_off.alloc(V + 1ull)) return -1;
   SB_CUDA_CHECK(cudaMemcpy(e->d_tok_bytes, tok_bytes, tok_off[V], cudaMemcpyHostToDevice));
   SB_CUDA_CHECK(cudaMemcpy(e->d_tok_off, tok_off, (V + 1) * 4ull, cudaMemcpyHostToDevice));
   return 0;

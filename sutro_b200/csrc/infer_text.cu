@@ -14,26 +14,11 @@
 
 #include "../../include/sutro_b200.h"
 #include "common.cuh"
+#include "dev_buf.h"
 #include "kernels.h"
 
 namespace sb {
 namespace {
-
-// device allocation that frees itself on every return path
-struct DevBuf {
-  void* p = nullptr;
-  ~DevBuf() {
-    if (p) cudaFree(p);
-  }
-  int alloc(size_t bytes) {
-    SB_CUDA_CHECK(cudaMalloc(&p, bytes ? bytes : 1));
-    return 0;
-  }
-  template <class T>
-  T* as() const {
-    return static_cast<T*>(p);
-  }
-};
 
 // three phases of the one-call path, timed with CUDA events on the engine's stream
 struct PhaseEvents {

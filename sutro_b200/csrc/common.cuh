@@ -259,6 +259,19 @@ SB_DEVICE uint32_t ld_shared_b32(uint32_t addr) {
   asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
   return v;
 }
+SB_DEVICE uint4 ld_shared_v4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+               : "r"(addr)
+               : "memory");
+  return v;
+}
+SB_DEVICE void st_shared_v4(uint32_t addr, const uint4& v) {
+  asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z),
+               "r"(v.w)
+               : "memory");
+}
 // 1-D bulk copy global -> shared (no tensor map; size multiple of 16 B).
 SB_DEVICE void bulk_load_1d(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
   asm volatile(

@@ -9,15 +9,21 @@
 //   warps 0-7  two consumer warpgroups: warpgroup c owns rows [64c, 64c+64) of the 128-row
 //              tile and issues wgmma.m64nBLOCK_Nk16 (four per 64-element K block) straight
 //              from the shared-memory ring, accumulating in registers; one K block stays in
-//              flight while the next is issued.  The fused epilogue rounds the registers into
-//              the warpgroup's 64-row slab of a staging buffer, and one thread stores the slab
-//              with TMA; the warpgroup goes on to the next tile's mainloop while it drains.
+//              flight while the next is issued.  The accumulators are rounded into the
+//              warpgroup's 64-row slab of a staging buffer.  For the store and residual
+//              epilogues the warpgroup finishes the slab itself and one thread stores it with
+//              TMA; for SwiGLU and QKV (a CTA with more than one tile, K >= 2048) it writes
+//              bf16(acc) and hands the slab to the epilogue warps.  Either way it goes on to the
+//              next tile's mainloop while the slab drains.
 //   warps 8-11 producer warpgroup (gives its registers to the consumers); warp 8 issues the
 //              cp.async.bulk.tensor 2-D loads of A (128x64) and W (BLOCK_N x 64) tiles into a
 //              kStages-deep ring and runs ahead into the next tile while the consumers are in
 //              their epilogue.  For RESIDUAL_BF16, warp 9 loads each slab's residual tile into
 //              the staging buffer by TMA as soon as the slab's previous store has read it out,
-//              so the load overlaps the tile's mainloop.
+//              so the load overlaps the tile's mainloop.  For SwiGLU and QKV, warps 9-11 are
+//              the epilogue warps: they run the epilogue math in place in each handed-over slab
+//              and store it, under the consumers' next mainloop (slab_full / slab_free
+//              mbarriers pass each slab back and forth).
 //
 // Fused epilogues (rounding points mirror the bf16 oracle, oracle/model_ref.py):
 //   STORE_BF16     D = bf16(acc)
@@ -107,6 +113,12 @@ SB_DEVICE void tile_to_mn(int GM, int tile, int num_m, int num_n, int& m_blk, in
 // The thread's accumulators: acc[4j + 2h + e] is row 8h of the thread's rows, column
 // 8j + 2 * (lane % 4) + e of the tile.
 
+// bf16(silu(g) * u) of the bf16-rounded gate and up values
+SB_DEVICE uint16_t swiglu_bf16(float g, float u) {
+  const float s = bf16_round(g / (1.0f + __expf(-g)));
+  return __bfloat16_as_ushort(__float2bfloat16_rn(s * u));
+}
+
 // STORE_BF16, SWIGLU_BF16, RESIDUAL_BF16 -> the warpgroup's staging slab; srow is the slab row
 // of the thread's first row, q = lane % 4.  For RESIDUAL_BF16 the slab already holds R (loaded
 // by TMA), which is read and overwritten in place: D = bf16(bf16(acc) + R).
@@ -120,11 +132,8 @@ SB_DEVICE void epilogue_stage(const float (&acc)[BLOCK_N / 2], uint32_t slab, in
       const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
       if constexpr (EPI == EPI_SWIGLU_BF16) {
         // gate/up columns 2c, 2c + 1 give output column c = 4j + q
-        const float g = bf16_round(v0);
-        const float u = bf16_round(v1);
-        const float s = bf16_round(g / (1.0f + __expf(-g)));
         st_shared_b16(slab + stage_off<Epi::kBoxCols>(srow + 8 * h, 4 * j + q),
-                      __bfloat16_as_ushort(__float2bfloat16_rn(s * u)));
+                      swiglu_bf16(bf16_round(v0), bf16_round(v1)));
       } else {
         const uint32_t a = slab + stage_off<64>(srow + 8 * h, 8 * j + 2 * q);
         if constexpr (EPI == EPI_RESIDUAL_BF16) {
@@ -180,10 +189,14 @@ SB_DEVICE void qkv_row_meta(const QkvEpiArgs& ea, int row, bool row_ok, QkvRowMe
   }
 }
 
-template <int R>
-SB_DEVICE void qkv_head_epilogue(const float (&acc)[R], int hh, const QkvEpiArgs& ea,
-                                 const QkvRowMeta (&rm)[2], int row0, int M, int head, bool head_ok,
-                                 uint32_t slab, int srow) {
+// One row of one head.  u[jj] holds dims 8jj + 2q, +1 of the head (q = lane % 4; the quad holds
+// the row's 128 dims), the bf16 rounding of the projection.  The result goes to the staging slab
+// at (srow, col0 + d) and, for a k/v head, to the row's KV page.  Every lane of the warp calls it
+// (the sum of squares is reduced over the quad); with ok = false (row >= M, or a head past N) it
+// writes nothing.
+SB_DEVICE void qkv_head_epilogue(const uint32_t (&u)[16], const QkvEpiArgs& ea,
+                                 const QkvRowMeta& rm, int head, bool ok, uint32_t slab, int srow,
+                                 int col0) {
   const int q = threadIdx.x & 3;
   const bool is_q = head < ea.hq;
   const bool is_k = !is_q && head < ea.hq + ea.hkv;
@@ -208,69 +221,148 @@ SB_DEVICE void qkv_head_epilogue(const float (&acc)[R], int hh, const QkvEpiArgs
     asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
     return d;
   };
+  float ss = 0.f;
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = row0 + 8 * h;
-    // 32 fp32 accumulators -> 16 packed bf16x2 (the rounding of the linear output):
-    // u[jj] holds dims 8jj + 2q, +1 of the head
-    uint32_t u[16];
-    float ss = 0.f;
+  for (int jj = 0; jj < 16; ++jj) {
+    const float2 f = unpack_bf16x2(u[jj]);
+    ss += f.x * f.x + f.y * f.y;
+  }
+  ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+  ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+  if (!ok) return;
+  const float rstd = nw != nullptr ? rsqrtf(ss / static_cast<float>(kHeadDim) + ea.eps) : 1.f;
+  // K/V page row; chunk c of the row is stored at c ^ swz: kv_chunk(r, c) == c ^ kv_chunk(r, 0),
+  // taken out of the loop below
+  __nv_bfloat16* kv_lo = nullptr;
+  int swz = 0;
+  if (!is_q) {
+    const int kvh = is_k ? (head - ea.hq) : (head - ea.hq - ea.hkv);
+    kv_lo = static_cast<__nv_bfloat16*>(ea.kv_layer) +
+            kv_tile_offset(rm.page, ea.hkv, kvh, is_k) + rm.r * kHeadDim;
+    swz = kv_chunk(rm.r, 0);
+  }
+  const __nv_bfloat16* cosr =
+      static_cast<const __nv_bfloat16*>(ea.cos_tab) + static_cast<size_t>(rm.pos) * 64;
+  const __nv_bfloat16* sinr =
+      static_cast<const __nv_bfloat16*>(ea.sin_tab) + static_cast<size_t>(rm.pos) * 64;
 #pragma unroll
-    for (int jj = 0; jj < 16; ++jj) {
-      const int i = 4 * (16 * hh + jj) + 2 * h;
-      u[jj] = pack_bf16x2(acc[i], acc[i + 1]);
-      const float2 f = unpack_bf16x2(u[jj]);
-      ss += f.x * f.x + f.y * f.y;
+  for (int jj = 0; jj < 8; ++jj) {   // dims d, d+1 of the low half and their +64 partners
+    const int d = 8 * jj + 2 * q;
+    uint32_t lo = u[jj], hi = u[jj + 8];
+    if (nw != nullptr) {   // w * bf16(x * rstd): rstd is fp32, so that product is fp32
+      const float2 a = unpack_bf16x2(lo), b = unpack_bf16x2(hi);
+      lo = mul2(*reinterpret_cast<const uint32_t*>(nw + d), pack_bf16x2(a.x * rstd, a.y * rstd));
+      hi = mul2(*reinterpret_cast<const uint32_t*>(nw + 64 + d),
+                pack_bf16x2(b.x * rstd, b.y * rstd));
     }
-    ss += __shfl_xor_sync(0xffffffffu, ss, 1);
-    ss += __shfl_xor_sync(0xffffffffu, ss, 2);
-    if (!head_ok || row >= M) continue;
-    const float rstd = nw != nullptr ? rsqrtf(ss / static_cast<float>(kHeadDim) + ea.eps) : 1.f;
-    // K/V page row; chunk c of the row is stored at c ^ swz: kv_chunk(r, c) == c ^ kv_chunk(r, 0),
-    // taken out of the loop below
-    __nv_bfloat16* kv_lo = nullptr;
-    int swz = 0;
+    if (is_q || is_k) {
+      // out[i] = x[i]*cos - x[i+64]*sin ; out[i+64] = x[i+64]*cos + x[i]*sin (bf16 op by op)
+      const uint32_t c = *reinterpret_cast<const uint32_t*>(cosr + d);
+      const uint32_t s = *reinterpret_cast<const uint32_t*>(sinr + d);
+      const uint32_t x = lo, y = hi;
+      lo = sub2(mul2(x, c), mul2(y, s));
+      hi = add2(mul2(y, c), mul2(x, s));
+    }
+    st_shared_b32(slab + stage_off<64>(srow, col0 + d), lo);
+    st_shared_b32(slab + stage_off<64>(srow, col0 + 64 + d), hi);
     if (!is_q) {
-      const int kvh = is_k ? (head - ea.hq) : (head - ea.hq - ea.hkv);
-      kv_lo = static_cast<__nv_bfloat16*>(ea.kv_layer) +
-              kv_tile_offset(rm[h].page, ea.hkv, kvh, is_k) + rm[h].r * kHeadDim;
-      swz = kv_chunk(rm[h].r, 0);
-    }
-    const __nv_bfloat16* cosr =
-        static_cast<const __nv_bfloat16*>(ea.cos_tab) + static_cast<size_t>(rm[h].pos) * 64;
-    const __nv_bfloat16* sinr =
-        static_cast<const __nv_bfloat16*>(ea.sin_tab) + static_cast<size_t>(rm[h].pos) * 64;
-#pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {   // dims d, d+1 of the low half and their +64 partners
-      const int d = 8 * jj + 2 * q;
-      uint32_t lo = u[jj], hi = u[jj + 8];
-      if (nw != nullptr) {   // w * bf16(x * rstd): rstd is fp32, so that product is fp32
-        const float2 a = unpack_bf16x2(lo), b = unpack_bf16x2(hi);
-        lo = mul2(*reinterpret_cast<const uint32_t*>(nw + d), pack_bf16x2(a.x * rstd, a.y * rstd));
-        hi = mul2(*reinterpret_cast<const uint32_t*>(nw + 64 + d),
-                  pack_bf16x2(b.x * rstd, b.y * rstd));
-      }
-      if (is_q || is_k) {
-        // out[i] = x[i]*cos - x[i+64]*sin ; out[i+64] = x[i+64]*cos + x[i]*sin (bf16 op by op)
-        const uint32_t c = *reinterpret_cast<const uint32_t*>(cosr + d);
-        const uint32_t s = *reinterpret_cast<const uint32_t*>(sinr + d);
-        const uint32_t x = lo, y = hi;
-        lo = sub2(mul2(x, c), mul2(y, s));
-        hi = add2(mul2(y, c), mul2(x, s));
-      }
-      st_shared_b32(slab + stage_off<64>(srow + 8 * h, 128 * hh + d), lo);
-      st_shared_b32(slab + stage_off<64>(srow + 8 * h, 128 * hh + 64 + d), hi);
-      if (!is_q) {
-        // the dense prefill attention reads the new tokens' K/V from the qkv buffer through TMA
-        // (attn_prefill_tc.cu); decode reads this paged copy
-        *reinterpret_cast<uint32_t*>(kv_lo + ((jj ^ swz) << 3) + 2 * q) = lo;
-        *reinterpret_cast<uint32_t*>(kv_lo + (((jj + 8) ^ swz) << 3) + 2 * q) = hi;
-      }
+      // the dense prefill attention reads the new tokens' K/V from the qkv buffer through TMA
+      // (attn_prefill_tc.cu); decode reads this paged copy
+      *reinterpret_cast<uint32_t*>(kv_lo + ((jj ^ swz) << 3) + 2 * q) = lo;
+      *reinterpret_cast<uint32_t*>(kv_lo + (((jj + 8) ^ swz) << 3) + 2 * q) = hi;
     }
   }
 }
 
+// ---------------------------------------------------------------------------
+// Epilogue warps (warps 9-11, SWIGLU_BF16 and QKV_ROPE): the consumers leave bf16(acc) in their
+// slab (the STORE_BF16 staging), and these 96 threads finish it in place.
+// ---------------------------------------------------------------------------
+constexpr int kEpiWarp0 = kProducerWarp + 1;
+constexpr int kEpiThreads = 96;
+constexpr int kEpiBar = 3;       // named barrier of the epilogue warps (1, 2: the consumers')
+constexpr int kQkvPasses = 3;    // 24 quads x 3 passes cover the slab's 64 rows
+
+// The slab row of epilogue quad `quad` (0..23) in pass i; rows >= 64 (the whole of warp 11 in
+// the last pass) have no work.
+SB_DEVICE int qkv_pass_row(int i, int quad) { return 24 * i + quad; }
+
+// QKV_ROPE: quad g takes slab rows g, g + 24, g + 48 and, in each, every head of the tile; lane
+// q loads the 16 words the consumer layout gives lane q, so qkv_head_epilogue sees the same
+// values in the same lanes.  Every lane reads its words before it writes them back, and no lane
+// touches another's.
+template <int BLOCK_N>
+SB_DEVICE void qkv_slab_epilogue(const QkvEpiArgs& ea, const QkvRowMeta (&rm)[kQkvPasses],
+                                 uint32_t slab, int row_base, int n_blk, int M, int N, int et) {
+  const int quad = et >> 2, q = et & 3;
+#pragma unroll
+  for (int i = 0; i < kQkvPasses; ++i) {
+    const int srow = qkv_pass_row(i, quad);
+    if (srow >= 64) continue;   // warp-uniform
+#pragma unroll
+    for (int hh = 0; hh < BLOCK_N / 128; ++hh) {
+      const int head = (n_blk * BLOCK_N) / kHeadDim + hh;
+      uint32_t u[16];
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj)
+        u[jj] = ld_shared_b32(slab + stage_off<64>(srow, 128 * hh + 8 * jj + 2 * q));
+      qkv_head_epilogue(u, ea, rm[i], head, head * kHeadDim < N && row_base + srow < M, slab,
+                        srow, 128 * hh);
+    }
+  }
+}
+
+// SWIGLU_BF16: item (row r, k) turns input columns [16k, 16k + 16) (8 interleaved gate/up pairs)
+// into output columns [8k, 8k + 8), one 16-byte chunk.  The output overwrites the input in place:
+// output chunk k of row r lies on input chunk k of row r (BLOCK_N >= 128) or on input row r / 2
+// (BLOCK_N = 64, 64-byte output rows), which items of the same or an earlier row read.  So the
+// items run in row-major passes, and in each pass every input is read before the barrier and
+// every output written after it.
+template <int BLOCK_N>
+SB_DEVICE void swiglu_slab_epilogue(uint32_t slab, int et) {
+  using Epi = EpiCfg<BLOCK_N, EPI_SWIGLU_BF16>;
+  constexpr int kChunks = BLOCK_N / 16;   // output chunks per row
+  constexpr int kItems = 64 * kChunks;
+  auto pair = [](uint32_t w0, uint32_t w1) {
+    const float2 a = unpack_bf16x2(w0), b = unpack_bf16x2(w1);
+    return static_cast<uint32_t>(swiglu_bf16(a.x, a.y)) |
+           (static_cast<uint32_t>(swiglu_bf16(b.x, b.y)) << 16);
+  };
+#pragma unroll 1
+  for (int base = 0; base < kItems; base += kEpiThreads) {
+    const int item = base + et;
+    const int r = item / kChunks, k = item % kChunks;
+    uint4 in0, in1;
+    if (item < kItems) {
+      in0 = ld_shared_v4(slab + stage_off<64>(r, 16 * k));
+      in1 = ld_shared_v4(slab + stage_off<64>(r, 16 * k + 8));
+    }
+    named_bar_sync(kEpiBar, kEpiThreads);
+    if (item < kItems)
+      st_shared_v4(slab + stage_off<Epi::kBoxCols>(r, 8 * k),
+                   make_uint4(pair(in0.x, in0.y), pair(in0.z, in0.w), pair(in1.x, in1.y),
+                              pair(in1.z, in1.w)));
+  }
+}
+
+// TMA store of one staged slab (rows [row, row + 64) of the tile) into the thread's bulk group.
 template <int BLOCK_N, int EPI>
+SB_DEVICE void store_slab(const CUtensorMap* tm_d, uint32_t slab, int row, int n_blk, int M,
+                          int N, const QkvEpiArgs& ea) {
+  using Epi = EpiCfg<BLOCK_N, EPI>;
+  const int n_out = EPI == EPI_SWIGLU_BF16 ? N / 2 : N;
+  for (int b = 0; b < Epi::kBoxes; ++b) {
+    const int col = n_blk * Epi::kCols + b * Epi::kBoxCols;
+    // decode (write_dense = 0) leaves the K/V columns of the qkv buffer untouched
+    const bool want = EPI != EPI_QKV_ROPE || ea.write_dense || col / kHeadDim < ea.hq;
+    if (row < M && col < n_out && want) tma_store_2d(tm_d, slab + b * Epi::kBoxBytes, col, row);
+  }
+  bulk_commit_group();
+}
+
+// EPI_WARPS (SWIGLU_BF16 and QKV_ROPE only): the epilogue warps finish and store each slab, and
+// the consumers only write bf16(acc); otherwise the consumers run the whole epilogue.
+template <int BLOCK_N, int EPI, bool EPI_WARPS>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
                     const __grid_constant__ CUtensorMap tm_b,
@@ -281,6 +373,15 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
   using Cfg = GemmCfg<BLOCK_N>;
   using Epi = EpiCfg<BLOCK_N, EPI>;
   constexpr bool kStaged = EPI != EPI_STORE_F32;
+  static_assert(!EPI_WARPS || EPI == EPI_SWIGLU_BF16 || EPI == EPI_QKV_ROPE,
+                "epilogue warps run SwiGLU and QKV only");
+  // setmaxnreg moves registers between the warpgroups within what the block was launched with
+  // (168 per thread, from __launch_bounds__): 2 x consumer + producer <= 3 x 168, or the
+  // consumers' setmaxnreg.inc waits forever.  The epilogue warps need more than the loaders, the
+  // consumers' bf16 store less than the fused math they no longer run.
+  constexpr int kProducerRegs = EPI_WARPS ? 120 : 40;
+  constexpr int kConsumerRegs = EPI_WARPS ? 192 : 232;
+  static_assert(2 * kConsumerRegs + kProducerRegs <= 3 * 168, "registers of the block");
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.
   uint8_t* smem = reinterpret_cast<uint8_t*>(
@@ -291,6 +392,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
   uint64_t* empty_bar = bars + Cfg::kStages;
   uint64_t* slab_free = bars + 2 * Cfg::kStages;   // per slab: its last store has read it out
   uint64_t* resid_full = slab_free + 2;            // per slab: the tile's residual has landed
+  uint64_t* slab_full = resid_full + 2;            // per slab: bf16(acc) is staged (EPI_WARPS)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -307,6 +409,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
     for (int c = 0; c < 2; ++c) {
       mbar_init(smem_u32(&slab_free[c]), 1);
       mbar_init(smem_u32(&resid_full[c]), 1);
+      if constexpr (EPI_WARPS) mbar_init(smem_u32(&slab_full[c]), kConsumerWarps / 2);
     }
     fence_mbar_init();
   }
@@ -319,7 +422,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
 
   if (warp >= kProducerWarp) {
     // ===== TMA producer =====
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<kProducerRegs>();
     if (warp == kProducerWarp && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -359,12 +462,48 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
             tma_load_2d(dst + b * Epi::kBoxBytes, &tm_r, bar, n_blk * BLOCK_N + 64 * b, row);
         }
       }
+    } else if (EPI_WARPS && warp >= kEpiWarp0) {
+      // epilogue warps: each slab as the consumers hand it over (slab_full), in tile order;
+      // once its stores have read it out, it goes back to them (slab_free)
+      const int et = threadIdx.x - 32 * kEpiWarp0;
+      uint32_t it = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+        int m_blk, n_blk;
+        tile_to_mn(ea_gm, tile, num_m, num_n, m_blk, n_blk);
+        for (int c = 0; c < 2; ++c) {
+          const int row_base = m_blk * kBlockM + 64 * c;
+          const uint32_t slab = smem_u32(staging + c * Cfg::kSlabBytes);
+          QkvRowMeta rm[kQkvPasses];
+          if constexpr (EPI == EPI_QKV_ROPE) {   // overlaps the wait for the slab
+#pragma unroll
+            for (int i = 0; i < kQkvPasses; ++i) {
+              const int srow = qkv_pass_row(i, et >> 2);
+              qkv_row_meta(ea, row_base + srow, srow < 64 && row_base + srow < M, rm[i]);
+            }
+          }
+          mbar_wait_long(smem_u32(&slab_full[c]), it & 1);
+          if constexpr (EPI == EPI_QKV_ROPE) {
+            qkv_slab_epilogue<BLOCK_N>(ea, rm, slab, row_base, n_blk, M, N, et);
+          } else {
+            swiglu_slab_epilogue<BLOCK_N>(slab, et);
+          }
+          fence_proxy_async_smem();   // this thread's slab writes, before the async proxy reads them
+          named_bar_sync(kEpiBar, kEpiThreads);
+          if (et == 0) {
+            store_slab<BLOCK_N, EPI>(&tm_d, slab, row_base, n_blk, M, N, ea);
+            bulk_wait_group_read<0>();
+            mbar_arrive(smem_u32(&slab_free[c]));
+          }
+        }
+      }
+      // the stores must finish reading shared memory before the block exits
+      if (et == 0) bulk_wait_group<0>();
     }
     return;
   }
 
   // ===== consumers: MMA + epilogue =====
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<kConsumerRegs>();
   const int wg = warp >> 2;   // rows [64 wg, 64 wg + 64) of the tile
   const uint32_t smem0 = smem_u32(smem);
   const uint32_t slab = smem_u32(staging + wg * Cfg::kSlabBytes);
@@ -379,7 +518,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
     tile_to_mn(ea_gm, tile, num_m, num_n, m_blk, n_blk);
     const int row0 = m_blk * kBlockM + wg * 64 + srow;
     QkvRowMeta rm[2];
-    if constexpr (EPI == EPI_QKV_ROPE) {   // overlaps the mainloop's loads
+    if constexpr (EPI == EPI_QKV_ROPE && !EPI_WARPS) {   // overlaps the mainloop's loads
       qkv_row_meta(ea, row0, row0 < M, rm[0]);
       qkv_row_meta(ea, row0 + 8, row0 + 8 < M, rm[1]);
     }
@@ -426,6 +565,15 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
       epilogue_store_f32<BLOCK_N>(acc, d_f32, row0, n_blk * BLOCK_N + 2 * (lane & 3), M, N, ldd);
       continue;
     }
+    if constexpr (EPI_WARPS) {
+      // the epilogue warps hand the slab back once its previous store has read it out; stage
+      // bf16(acc), hand it over and go straight into the next tile
+      mbar_wait(smem_u32(&slab_free[wg]), (it & 1) ^ 1);
+      epilogue_stage<BLOCK_N, EPI_STORE_BF16>(acc, slab, srow, lane & 3);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(&slab_full[wg]));
+      continue;
+    }
     if constexpr (EPI == EPI_RESIDUAL_BF16) {
       mbar_wait(smem_u32(&resid_full[wg]), it & 1);
     } else {
@@ -438,27 +586,29 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tm_a,
 #pragma unroll
       for (int hh = 0; hh < BLOCK_N / 128; ++hh) {
         const int head = (n_blk * BLOCK_N) / kHeadDim + hh;
-        qkv_head_epilogue(acc, hh, ea, rm, row0, M, head, head * kHeadDim < N, slab, srow);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          // 32 fp32 accumulators -> 16 packed bf16x2 (the rounding of the linear output):
+          // u[jj] holds dims 8jj + 2q, +1 of the head
+          uint32_t u[16];
+#pragma unroll
+          for (int jj = 0; jj < 16; ++jj) {
+            const int i = 4 * (16 * hh + jj) + 2 * h;
+            u[jj] = pack_bf16x2(acc[i], acc[i + 1]);
+          }
+          qkv_head_epilogue(u, ea, rm[h], head, head * kHeadDim < N && row0 + 8 * h < M, slab,
+                            srow + 8 * h, 128 * hh);
+        }
       }
     } else {
       epilogue_stage<BLOCK_N, EPI>(acc, slab, srow, lane & 3);
     }
     fence_proxy_async_smem();   // this thread's slab writes, before the async proxy reads them
     named_bar_sync(1 + wg, 128);
-    if (leader) {
-      const int row = m_blk * kBlockM + 64 * wg;
-      const int n_out = EPI == EPI_SWIGLU_BF16 ? N / 2 : N;
-      for (int b = 0; b < Epi::kBoxes; ++b) {
-        const int col = n_blk * Epi::kCols + b * Epi::kBoxCols;
-        // decode (write_dense = 0) leaves the K/V columns of the qkv buffer untouched
-        const bool want = EPI != EPI_QKV_ROPE || ea.write_dense || col / kHeadDim < ea.hq;
-        if (row < M && col < n_out && want) tma_store_2d(&tm_d, slab + b * Epi::kBoxBytes, col, row);
-      }
-      bulk_commit_group();
-    }
+    if (leader) store_slab<BLOCK_N, EPI>(&tm_d, slab, m_blk * kBlockM + 64 * wg, n_blk, M, N, ea);
   }
   // the stores must finish reading shared memory before the block exits
-  if (kStaged && leader) bulk_wait_group<0>();
+  if (kStaged && !EPI_WARPS && leader) bulk_wait_group<0>();
 }
 
 // ---------------------------------------------------------------------------
@@ -637,10 +787,23 @@ int raster_group(int tile_rows, int N, int K) {
   return static_cast<int>(gm);
 }
 
+template <int BLOCK_N, int EPI, bool EPI_WARPS>
+int launch_kernel(int grid, cudaStream_t stream, const CUtensorMap& tm_a, const CUtensorMap& tm_b,
+                   const CUtensorMap& tm_d, const CUtensorMap& tm_r, void* d, int M, int N, int K,
+                   int ldd, int gm, const QkvEpiArgs& ea) {
+  using Cfg = GemmCfg<BLOCK_N>;
+  auto kern = gemm_bf16_tn_kernel<BLOCK_N, EPI, EPI_WARPS>;
+  SB_SET_MAX_SMEM(kern, Cfg::kSmemBytes);
+  kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(tm_a, tm_b, tm_d, tm_r,
+                                                        reinterpret_cast<float*>(d), M, N, K, ldd,
+                                                        gm, ea);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
 template <int BLOCK_N, int EPI>
 int launch_cfg(const void* a, int a_rows, const void* w, void* d, const void* resid, int M, int N,
                int K, int ldd, cudaStream_t stream, const QkvEpiArgs& ea) {
-  using Cfg = GemmCfg<BLOCK_N>;
   CUtensorMap tm_a, tm_b, tm_d{}, tm_r{};
   if (make_tmap(a, a_rows, K, kBlockM, &tm_a)) return -1;
   if (make_tmap(w, N, K, BLOCK_N, &tm_b)) return -1;
@@ -650,15 +813,21 @@ int launch_cfg(const void* a, int a_rows, const void* w, void* d, const void* re
       return -1;
     if (EPI == EPI_RESIDUAL_BF16 && make_epi_tmap(resid, M, N, ldd, 64, &tm_r)) return -1;
   }
-  auto kern = gemm_bf16_tn_kernel<BLOCK_N, EPI>;
-  SB_SET_MAX_SMEM(kern, Cfg::kSmemBytes);
   const int tiles = ((M + kBlockM - 1) / kBlockM) * ((N + BLOCK_N - 1) / BLOCK_N);
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  kern<<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(
-      tm_a, tm_b, tm_d, tm_r, reinterpret_cast<float*>(d), M, N, K, ldd,
-      raster_group(kBlockM, N, K), ea);
-  SB_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  const int gm = raster_group(kBlockM, N, K);
+  // The epilogue warps hide the SwiGLU / QKV math under the next tile's mainloop.  A CTA with
+  // one tile has no next mainloop, and there the eight consumer warps finish the math sooner
+  // (M = 128: 0.119 against 0.131 ms for the four qwen-3-4b shapes).  The math per tile is fixed
+  // while the mainloop grows with K: at K = 2,560 it hides under it, at K = 1,024
+  // (qwen-3-embedding-0.6b) three warps fall behind and the GEMMs slow down.
+  if constexpr (EPI == EPI_SWIGLU_BF16 || EPI == EPI_QKV_ROPE) {
+    if (tiles > grid && K >= 2048)
+      return launch_kernel<BLOCK_N, EPI, true>(grid, stream, tm_a, tm_b, tm_d, tm_r, d, M, N, K,
+                                               ldd, gm, ea);
+  }
+  return launch_kernel<BLOCK_N, EPI, false>(grid, stream, tm_a, tm_b, tm_d, tm_r, d, M, N, K, ldd,
+                                            gm, ea);
 }
 
 template <int EPI>

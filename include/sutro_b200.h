@@ -117,7 +117,9 @@ int sb200_fsm_build_mask(const int32_t* fsm_trans, const uint8_t* fsm_accept, in
                          const uint8_t* tok_bytes, const int32_t* tok_off, int vocab, int eos_id,
                          uint32_t* mask_bits, int mask_words, void* stream);
 
-/* Test hook: one sampling step (K8) exactly as the engine runs it on a chunk of logits rows.
+/* Test hook: one sampling step (K8) exactly as the engine runs it on a chunk of logits rows:
+ * the penalty kernel when a penalty is active (it rewrites `logits` in place), then the greedy or
+ * the stochastic kernel.
  * The fields mirror the engine's internal arguments one for one; every pointer is a device
  * pointer.  Values are used as given: temperature <= 0 runs the greedy kernel (arg-max, lowest
  * index wins ties), top_k <= 0 and top_p >= 1 switch those filters off (the engine's
@@ -128,7 +130,7 @@ int sb200_fsm_build_mask(const int32_t* fsm_trans, const uint8_t* fsm_accept, in
  * then exactly {allowed i : key(z_i) >= out_tau}.  Not written by the greedy kernel, nor for
  * rows where nothing is selectable. */
 typedef struct {
-  const float* logits;      /* [B, ldl] fp32                                                */
+  float* logits;            /* [B, ldl] fp32; rewritten in place when a penalty is active   */
   int ldl, vocab, B;
   const int32_t* row_slot;  /* [B] slot of each logits row                                  */
   int32_t* slot_state;      /* per slot: DFA state, -1 = unconstrained (NULL = all -1)      */
@@ -160,6 +162,18 @@ typedef struct {
   float* slot_cum_logprob;   /* optional: running sum of log p(token)                       */
   float* out_cum_logprob;    /* optional [n_rows]                                           */
   uint32_t* out_tau;         /* optional [B], see above                                     */
+  /* as in sb200_job (0 = off; repetition_penalty <= 0 is off too); min_p raises out_tau     */
+  float presence_penalty, frequency_penalty, repetition_penalty, min_p;
+  /* the prompt the penalties count, needed when one is active: prompt_prefix |
+   * row_tokens[row_tok_off[row] ..][0, slot_n_row_tok[slot]) | prompt_suffix, row =
+   * slot_row[slot]; the output is out_tokens[row][0, slot_ngen[slot]); out_stride <= 8192    */
+  const int32_t* prompt_prefix;
+  int n_prompt_prefix;
+  const int32_t* prompt_suffix;
+  int n_prompt_suffix;
+  const int32_t* row_tokens;
+  const int64_t* row_tok_off;
+  const int32_t* slot_n_row_tok;
 } sb200_sample_args;
 
 int sb200_sample(const sb200_sample_args* args, void* stream);
@@ -279,6 +293,18 @@ typedef struct {
                                      stream when seed_per_row = 1 (the row's index in the whole
                                      job when the job is sharded over GPUs, so that draws do not
                                      depend on the sharding); NULL = the local row index       */
+  /* vLLM's sampling_params of the same names; zero = off.  Penalties apply, in vLLM's order, to
+   * greedy and sampled rows: repetition to every token of prompt ∪ output (l * 1/r when l > 0,
+   * else l * r), then l -= frequency_penalty * count and l -= presence_penalty for every token of
+   * the output (count = its occurrences).  The prompt is prefix | row tokens after truncation |
+   * suffix; the output is what the row has generated, the jump-forward prefix included.  With a
+   * penalty active, max_new_tokens may be at most 8192.  min_p (sampled rows only, applied before
+   * top_k / top_p): keep z >= max z + ln(min_p).  Cumulative log-probabilities are taken over the
+   * penalised logits; out_first_logits_dev keeps the raw ones.                               */
+  float presence_penalty;         /* [-2, 2]                                             */
+  float frequency_penalty;        /* [-2, 2]                                             */
+  float repetition_penalty;       /* > 0; 1 and <= 0 are off                              */
+  float min_p;                    /* [0, 1]                                              */
 } sb200_job;
 
 /* kernel classes for the per-class launch counts / device times in sb200_job_stats */
@@ -396,7 +422,8 @@ int64_t sb200_schema_longest_path(void* schema);
  * jump-forward plan from the automaton, picks max_new_tokens when <= 0 (the longest string the
  * schema admits, else 512; capped at half the context window) and runs sb200_infer_text on the
  * rows.  `sampling` may be NULL (greedy); only its temperature / top_k / top_p / seed /
- * seed_per_row / ignore_eos / truncate_rows / progress fields are read.
+ * seed_per_row / ignore_eos / truncate_rows / progress / profile / presence_penalty /
+ * frequency_penalty / repetition_penalty / min_p fields are read.
  * ---------------------------------------------------------------------- */
 int sb200_model_open(const char* bundle_dir, int device, int max_slots, int max_prefill_tokens,
                      int64_t kv_pages, void** out_model);

@@ -5,9 +5,10 @@ duck-typed (pandas always available, polars / pyarrow when installed).
 """
 from __future__ import annotations
 
+import math
 import os
 import sys
-from typing import Any, Dict, List, Literal, Type, Union
+from typing import Any, Dict, List, Literal, Tuple, Type, Union
 
 import pandas as pd
 
@@ -172,3 +173,20 @@ def normalize_output_schema(output_schema: Union[Dict[str, Any], Type[Any], None
     if isinstance(output_schema, dict):
         return output_schema
     raise ValueError("Invalid output schema type. Must be a dictionary or a pydantic Model.")
+
+
+def check_penalties(presence_penalty=0.0, frequency_penalty=0.0, repetition_penalty=1.0,
+                    min_p=0.0) -> Tuple[float, float, float, float]:
+    """vLLM's ranges for its sampling parameters of the same names (ValueError outside them);
+    returns them as floats.  Neutral: presence 0, frequency 0, repetition 1, min_p 0."""
+    p, f, r, m = (float(x) for x in (presence_penalty, frequency_penalty, repetition_penalty,
+                                     min_p))
+    if not -2.0 <= p <= 2.0:
+        raise ValueError(f"presence_penalty must be in [-2, 2], got {p}")
+    if not -2.0 <= f <= 2.0:
+        raise ValueError(f"frequency_penalty must be in [-2, 2], got {f}")
+    if not (r > 0.0 and math.isfinite(r)):
+        raise ValueError(f"repetition_penalty must be > 0, got {r}")
+    if not 0.0 <= m <= 1.0:
+        raise ValueError(f"min_p must be in [0, 1], got {m}")
+    return p, f, r, m

@@ -163,6 +163,17 @@ int sb200_sample(const sb200_sample_args* p, void* stream) {
   a.slot_cum_logprob = p->slot_cum_logprob;
   a.out_cum_logprob = p->out_cum_logprob;
   a.out_tau = p->out_tau;
+  a.presence_penalty = p->presence_penalty;
+  a.frequency_penalty = p->frequency_penalty;
+  a.repetition_penalty = p->repetition_penalty;
+  a.min_p = p->min_p;
+  a.prompt_prefix = p->prompt_prefix;
+  a.n_prompt_prefix = p->n_prompt_prefix;
+  a.prompt_suffix = p->prompt_suffix;
+  a.n_prompt_suffix = p->n_prompt_suffix;
+  a.row_tokens = p->row_tokens;
+  a.row_tok_off = p->row_tok_off;
+  a.slot_n_row_tok = p->slot_n_row_tok;
   return sample_greedy(a, STREAM(stream));
 }
 

@@ -66,7 +66,8 @@ init_slots_kernel(const SeqInit* __restrict__ seqs, const int32_t* __restrict__ 
                   int32_t* slot_ngen, int32_t* slot_pos, int32_t* slot_done, int32_t* slot_row,
                   int32_t* slot_maxnew, int32_t* slot_next_tok, const int32_t* __restrict__ forced,
                   int n_forced, int32_t* __restrict__ out_tokens, int32_t* __restrict__ out_len,
-                  int out_stride, float* __restrict__ slot_cum_logprob) {
+                  int out_stride, float* __restrict__ slot_cum_logprob,
+                  int32_t* __restrict__ slot_n_row_tok) {
   const SeqInit s = seqs[blockIdx.x];
   for (int i = threadIdx.x; i < max_pages; i += blockDim.x)
     page_table[static_cast<size_t>(s.slot) * max_pages + i] =
@@ -85,6 +86,7 @@ init_slots_kernel(const SeqInit* __restrict__ seqs, const int32_t* __restrict__ 
     slot_maxnew[s.slot] = s.max_new;
     slot_next_tok[s.slot] = 0;
     slot_cum_logprob[s.slot] = 0.f;
+    slot_n_row_tok[s.slot] = s.n_row_tok;  // the row's share of the prompt (penalties)
   }
 }
 
@@ -224,7 +226,7 @@ struct Engine {
   DevArray<float> logits, embed_tmp;
   DevArray<int32_t> tok_ids, tok_pos, tok_slot, ctx_len, row_slot, last_idx, page_table;
   DevArray<int32_t> slot_state, slot_ngen, slot_next_tok, slot_pos, slot_done, slot_row,
-      slot_maxnew;
+      slot_maxnew, slot_n_row_tok;
   DevArray<float> slot_cum_logprob;
   // Staging: a prefill step's StageLayout, or a decode step's row_slot.  The host buffer is
   // written only after the stream has been synchronised since its previous copy was enqueued:
@@ -284,7 +286,8 @@ struct Engine {
         ctx_len.alloc(S) || row_slot.alloc(S) || last_idx.alloc(S) ||
         page_table.alloc(S * max_pages) || slot_state.alloc(S) || slot_ngen.alloc(S) ||
         slot_next_tok.alloc(S) || slot_pos.alloc(S) || slot_done.alloc(S) ||
-        slot_row.alloc(S) || slot_maxnew.alloc(S) || slot_cum_logprob.alloc(S))
+        slot_row.alloc(S) || slot_maxnew.alloc(S) || slot_cum_logprob.alloc(S) ||
+        slot_n_row_tok.alloc(S))
       return -1;
     if (c.embedding_model) {
       if (embed_tmp.alloc(static_cast<size_t>(c.max_slots) * c.d_model)) return -1;
@@ -421,6 +424,19 @@ struct Engine {
       a.row_ids = job.row_ids_dev;
       a.slot_cum_logprob = job.out_cum_logprob_dev ? slot_cum_logprob.get() : nullptr;
       a.out_cum_logprob = job.out_cum_logprob_dev;
+      // penalties over prefix | row tokens after truncation | suffix and the row's output
+      a.prompt_prefix = d_prefix;
+      a.n_prompt_prefix = job.n_prefix;
+      a.prompt_suffix = d_suffix;
+      a.n_prompt_suffix = job.n_suffix;
+      a.row_tokens = job.row_tokens_dev;
+      a.row_tok_off = job.row_tok_off_dev;
+      a.slot_n_row_tok = slot_n_row_tok;
+      a.presence_penalty = job.presence_penalty;
+      a.frequency_penalty = job.frequency_penalty;
+      a.repetition_penalty = job.repetition_penalty;
+      a.min_p = job.min_p;
+      if (penalties_active(a)) ++prof.launches[SB200_KC_SAMPLE];  // the penalty kernel
       SB_K(SB200_KC_SAMPLE, sample_greedy(a, stream));
     }
     return 0;
@@ -479,6 +495,21 @@ int validate_job(const sb200_engine_config& c, const sb200_job& job, JobSpec& s)
                    : (job.out_tokens_dev == nullptr || job.out_len_dev == nullptr)) {
     set_last_error("engine: output buffers missing");
     return -1;
+  }
+  if (!s.embed_mode) {
+    const bool penalised = job.presence_penalty != 0.f || job.frequency_penalty != 0.f ||
+                           (job.repetition_penalty > 0.f && job.repetition_penalty != 1.f);
+    if (penalised && s.max_new > kPenaltyMaxOutput) {
+      set_last_error("engine: presence/frequency/repetition penalties support max_new_tokens <= "
+                     "%d (got %d)", kPenaltyMaxOutput, s.max_new);
+      return -1;
+    }
+    if (!(job.min_p <= 1.f) || !(job.presence_penalty == job.presence_penalty) ||
+        !(job.frequency_penalty == job.frequency_penalty) ||
+        !(job.repetition_penalty == job.repetition_penalty)) {
+      set_last_error("engine: min_p must be in [0, 1] and the penalties must be numbers");
+      return -1;
+    }
   }
   s.n_prefix = job.n_prefix;
   s.n_suffix = job.n_suffix;
@@ -669,7 +700,7 @@ struct JobRun {
         e.slot_done, e.slot_row, e.slot_maxnew, e.slot_next_tok,
         e.d_suffix + (p.n_suffix - p.n_forced), p.n_forced,
         p.embed_mode ? nullptr : job.out_tokens_dev, p.embed_mode ? nullptr : job.out_len_dev,
-        job.max_new_tokens, e.slot_cum_logprob);
+        job.max_new_tokens, e.slot_cum_logprob, e.slot_n_row_tok);
     prefill_prepare_kernel<<<n, 128, 0, e.stream>>>(d.seqs, e.d_prefix, p.n_prefix, e.d_suffix,
                                                     p.n_suffix, job.row_tokens_dev,
                                                     job.row_tok_off_dev, e.tok_ids, e.tok_pos,

@@ -113,7 +113,7 @@ int encode_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t
 
 // K8 — FSM token-mask build, masked greedy sampling + FSM advance.
 struct SampleArgs {
-  const float* logits;      // [B, ldl]
+  float* logits;            // [B, ldl]; rewritten in place when a penalty is active
   int ldl;
   int vocab;
   int B;
@@ -152,8 +152,24 @@ struct SampleArgs {
   float* out_cum_logprob;  // [n_rows], written together with out_len
   uint32_t* out_tau;       // nullable [B]: order-preserving key of the smallest kept z (stochastic
                            // kernel only; 0 = no filter).  Kept = allowed and fkey(z) >= tau.
+  // presence / frequency / repetition penalties (vLLM's apply_penalties) over the row's prompt
+  // prefix | row_tokens[row_tok_off[row] ..][0, slot_n_row_tok[slot]) | suffix and its output
+  // out_tokens[row][0, slot_ngen[slot]); min_p (stochastic kernel only).  0 = off, except
+  // repetition_penalty, where <= 0 and 1 are off.
+  const int32_t* prompt_prefix;
+  int n_prompt_prefix;
+  const int32_t* prompt_suffix;
+  int n_prompt_suffix;
+  const int32_t* row_tokens;
+  const int64_t* row_tok_off;
+  const int32_t* slot_n_row_tok;
+  float presence_penalty, frequency_penalty, repetition_penalty, min_p;
 };
-int sample_greedy(const SampleArgs& a, cudaStream_t stream);  // dispatches on a.temperature
+// The row-history table of the penalty kernel is sized by out_stride; longer outputs are refused.
+constexpr int kPenaltyMaxOutput = 8192;
+bool penalties_active(const SampleArgs& a);  // sample_greedy() then launches the penalty kernel
+// Penalties (when active), then the greedy or the stochastic kernel, dispatched on a.temperature.
+int sample_greedy(const SampleArgs& a, cudaStream_t stream);
 int prepare_decode(const int32_t* row_slot, const int32_t* slot_next_tok, const int32_t* slot_pos,
                    int32_t* tok_ids, int32_t* tok_pos, int32_t* tok_slot, int32_t* ctx_len, int B,
                    cudaStream_t stream);

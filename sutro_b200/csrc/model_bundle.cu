@@ -421,6 +421,10 @@ int sb200_model_infer(void* model, const char* system_prompt_utf8, const char* j
     job.ignore_eos = sampling->ignore_eos;
     job.progress = sampling->progress, job.progress_user = sampling->progress_user;
     job.profile = sampling->profile;
+    job.presence_penalty = sampling->presence_penalty;
+    job.frequency_penalty = sampling->frequency_penalty;
+    job.repetition_penalty = sampling->repetition_penalty;
+    job.min_p = sampling->min_p;
   }
   job.truncate_rows = sampling ? sampling->truncate_rows : 1;
   if (!sampling) job.truncate_rows = 1;

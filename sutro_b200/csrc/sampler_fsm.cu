@@ -7,10 +7,15 @@
 //                    index wins ties), append to the row's output, advance the
 //                    row's DFA state by the chosen token's bytes, raise the done
 //                    flag on EOS / final state / max_new_tokens.
-//   sample_random    temperature / top-k / top-p sampling under the same mask
+//   sample_random    temperature / min-p / top-k / top-p sampling under the same mask
 //                    (exact radix-select thresholds, Philox4x32-10 draws).
+//   apply_penalties  presence / frequency / repetition penalties on the logits, in place,
+//                    before either sampler (vLLM's semantics).
 //   prepare_decode   gathers next-step inputs (token, position, context length)
 //                    from the per-slot decode state, entirely on device.
+#include <algorithm>
+#include <cmath>
+
 #include "common.cuh"
 #include "kernels.h"
 
@@ -119,6 +124,104 @@ __device__ float block_sum(float v, float* sv) {
   return r;
 }
 
+// ---------------------------------------------------------------------------
+// presence / frequency / repetition penalties, in place on the fp32 logits, in vLLM's order
+// (vllm.model_executor.layers.utils.apply_penalties):
+//   l *= (l > 0 ? 1/r : r)       for every token of prompt ∪ output
+//   l -= f * count               count = occurrences in the output
+//   l -= p * (count > 0)
+// One CTA per row rebuilds the row's history table from its prompt pieces and out_tokens: a
+// bitmap of the prompt's tokens and a hash of the output's token counts, both in shared memory.
+// Every logit is then rewritten at most once, by the thread that owns its token, from the raw
+// logit, the count and the in-prompt bit alone, so the result does not depend on the order of
+// the atomics or on the batch.  The roundings are spelled out: l - f*c must not become an FMA.
+// ---------------------------------------------------------------------------
+constexpr int kPenaltyThreads = 256;
+
+struct PenaltyParams {
+  float rep, rep_inv, freq, pres;
+  int hash_size;   // power of two >= 2 * out_stride: the hash never fills
+  int zero_pass;   // f or p has its sign bit set: vLLM's l - (f*0) turns -0.0 into +0.0
+};
+
+__device__ __forceinline__ float penalize(float l, int count, bool seen, const PenaltyParams& q) {
+  if (seen) l = __fmul_rn(l, l > 0.f ? q.rep_inv : q.rep);
+  l = __fsub_rn(l, __fmul_rn(q.freq, static_cast<float>(count)));
+  return __fsub_rn(l, __fmul_rn(q.pres, count > 0 ? 1.f : 0.f));
+}
+
+__global__ void __launch_bounds__(kPenaltyThreads) apply_penalties_kernel(SampleArgs a,
+                                                                          PenaltyParams q) {
+  extern __shared__ uint32_t pen_smem[];
+  const int b = blockIdx.x;
+  const int slot = a.row_slot[b];
+  if (a.slot_done[slot]) return;
+  const int row = a.slot_row[slot];
+  const int V = a.vocab;
+  const int words = (V + 31) >> 5;
+  uint32_t* in_prompt = pen_smem;                                      // [words]
+  int32_t* hkey = reinterpret_cast<int32_t*>(pen_smem + words);        // [hash_size], -1 empty
+  int32_t* hcnt = hkey + q.hash_size;                                  // [hash_size]
+  const uint32_t hmask = static_cast<uint32_t>(q.hash_size - 1);
+  float* lg = a.logits + static_cast<size_t>(b) * a.ldl;
+  for (int i = threadIdx.x; i < words; i += kPenaltyThreads) in_prompt[i] = 0u;
+  for (int i = threadIdx.x; i < q.hash_size; i += kPenaltyThreads) hkey[i] = -1, hcnt[i] = 0;
+  __syncthreads();
+
+  // 1. the table: prompt bitmap, output counts
+  const int n_pre = a.n_prompt_prefix, n_row = a.slot_n_row_tok[slot], n_suf = a.n_prompt_suffix;
+  const int n_prompt = n_pre + n_row + n_suf;
+  const int32_t* row_toks = a.row_tokens + a.row_tok_off[row];
+  auto prompt_tok = [&](int j) {
+    return j < n_pre ? a.prompt_prefix[j]
+                     : (j < n_pre + n_row ? row_toks[j - n_pre] : a.prompt_suffix[j - n_pre - n_row]);
+  };
+  for (int j = threadIdx.x; j < n_prompt; j += kPenaltyThreads) {
+    const int t = prompt_tok(j);
+    if (t >= 0 && t < V) atomicOr(&in_prompt[t >> 5], 1u << (t & 31));
+  }
+  const int n_out = a.slot_ngen[slot];
+  const int32_t* out = a.out_tokens + static_cast<size_t>(row) * a.out_stride;
+  for (int j = threadIdx.x; j < n_out; j += kPenaltyThreads) {
+    const int t = out[j];
+    if (t < 0 || t >= V) continue;
+    for (uint32_t h = (static_cast<uint32_t>(t) * 2654435761u) & hmask;; h = (h + 1) & hmask) {
+      const int k = atomicCAS(&hkey[h], -1, t);
+      if (k == -1 || k == t) {
+        atomicAdd(&hcnt[h], 1);
+        break;
+      }
+    }
+  }
+  __syncthreads();
+
+  // 2. every output token, once (its hash entry); its prompt bit is taken so step 3 skips it
+  for (int h = threadIdx.x; h < q.hash_size; h += kPenaltyThreads) {
+    const int t = hkey[h];
+    if (t < 0) continue;
+    atomicAnd(&in_prompt[t >> 5], ~(1u << (t & 31)));
+    lg[t] = penalize(lg[t], hcnt[h], true, q);
+  }
+  __syncthreads();
+
+  // 3. every prompt token that is not in the output, once: the thread that clears its bit
+  for (int j = threadIdx.x; j < n_prompt; j += kPenaltyThreads) {
+    const int t = prompt_tok(j);
+    if (t < 0 || t >= V) continue;
+    const uint32_t bit = 1u << (t & 31);
+    if (atomicAnd(&in_prompt[t >> 5], ~bit) & bit) lg[t] = penalize(lg[t], 0, true, q);
+  }
+
+  // 4. the tokens outside the history: l - (f*0) - (p*0) is l, except that a negative f or p
+  //    (whose product with 0 is -0.0) turns -0.0 into +0.0.  A token steps 2-3 rewrote never
+  //    ends at -0.0 then, so this still rewrites every logit at most once.
+  if (q.zero_pass) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < V; i += kPenaltyThreads)
+      if (__float_as_uint(lg[i]) == 0x80000000u) lg[i] = 0.f;
+  }
+}
+
 __global__ void __launch_bounds__(kSampleThreads) sample_greedy_kernel(SampleArgs a) {
   const int b = blockIdx.x;
   const int slot = a.row_slot[b];
@@ -179,8 +282,10 @@ __device__ uint4 philox4x32_10(uint2 key, uint4 c) {
   return c;
 }
 
-// 4 CTAs per SM (32 registers): a 512-row chunk then runs in one wave on 132 SMs
-__global__ void __launch_bounds__(kSampleThreads, 4) sample_random_kernel(SampleArgs a) {
+// 4 CTAs per SM (32 registers): a 512-row chunk then runs in one wave on 132 SMs.
+// log_min_p = fp32(ln min_p), computed on the host; read only when a.min_p > 0.
+__global__ void __launch_bounds__(kSampleThreads, 4) sample_random_kernel(SampleArgs a,
+                                                                          float log_min_p) {
   const int b = blockIdx.x;
   const int slot = a.row_slot[b];
   if (a.slot_done[slot]) return;
@@ -202,6 +307,7 @@ __global__ void __launch_bounds__(kSampleThreads, 4) sample_random_kernel(Sample
   __shared__ unsigned long long sh_above, sh_target;
   __shared__ float wsum[kSampleWarps + 1];
   __shared__ int sh_tok;
+  __shared__ uint32_t sh_tau;
 
   // 1. max of z over the allowed tokens
   ArgMax m{-INFINITY, 0x7fffffff};
@@ -214,8 +320,12 @@ __global__ void __launch_bounds__(kSampleThreads, 4) sample_random_kernel(Sample
   }
   const float zmax = m.v;
 
-  // 2. top-k threshold (key of the k-th largest z), ties kept
-  uint32_t tau = 0;
+  // 2. min_p (vLLM v1: before top-k / top-p) keeps z >= zmax + ln(min_p); top-k keeps the z
+  //    >= the k-th largest (ties kept).  Every filter keeps an upper set of z, so their
+  //    intersection is the one with the largest threshold.
+  if (threadIdx.x == 0) sh_tau = a.min_p > 0.f ? fkey(__fadd_rn(zmax, log_min_p)) : 0u;
+  __syncthreads();
+  uint32_t tau = sh_tau;
   if (a.top_k > 0) {
     if (threadIdx.x == 0) sh_prefix = 0, sh_pmask = 0, sh_k = a.top_k;
     for (int shift = 24; shift >= 0; shift -= 8) {
@@ -244,7 +354,7 @@ __global__ void __launch_bounds__(kSampleThreads, 4) sample_random_kernel(Sample
       }
       __syncthreads();
     }
-    tau = sh_prefix;
+    tau = max(tau, sh_prefix);
     __syncthreads();  // every thread holds tau before the top-p descent reuses sh_prefix
   }
 
@@ -425,11 +535,50 @@ int fsm_build_mask(const int32_t* fsm_trans, const uint8_t* fsm_accept, int n_st
   return 0;
 }
 
+static float repetition_of(const SampleArgs& a) {
+  return a.repetition_penalty > 0.f ? a.repetition_penalty : 1.f;  // a zeroed struct: off
+}
+
+bool penalties_active(const SampleArgs& a) {
+  return a.presence_penalty != 0.f || a.frequency_penalty != 0.f || repetition_of(a) != 1.f;
+}
+
 int sample_greedy(const SampleArgs& a, cudaStream_t stream) {
   if (a.B <= 0) return 0;
-  if (a.temperature > 0.f)
-    sample_random_kernel<<<a.B, kSampleThreads, 0, stream>>>(a);
-  else
+  if (penalties_active(a)) {
+    if (a.out_stride > kPenaltyMaxOutput) {
+      set_last_error("sample: penalties support at most %d output tokens per row (max_new_tokens "
+                     "= %d)", kPenaltyMaxOutput, a.out_stride);
+      return -1;
+    }
+    if (a.slot_n_row_tok == nullptr || a.row_tokens == nullptr || a.row_tok_off == nullptr ||
+        (a.n_prompt_prefix > 0 && a.prompt_prefix == nullptr) ||
+        (a.n_prompt_suffix > 0 && a.prompt_suffix == nullptr)) {
+      set_last_error("sample: penalties need the rows' prompt tokens");
+      return -1;
+    }
+    PenaltyParams q;
+    q.rep = repetition_of(a);
+    q.rep_inv = 1.f / q.rep;
+    q.freq = a.frequency_penalty;
+    q.pres = a.presence_penalty;
+    q.hash_size = 32;
+    while (q.hash_size < 2 * a.out_stride) q.hash_size *= 2;
+    q.zero_pass = std::signbit(a.frequency_penalty) || std::signbit(a.presence_penalty);
+    const size_t smem = ((a.vocab + 31) / 32) * 4ull + q.hash_size * 8ull;
+    if (smem > 48 * 1024)
+      SB_CUDA_CHECK(cudaFuncSetAttribute(apply_penalties_kernel,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         static_cast<int>(smem)));
+    apply_penalties_kernel<<<a.B, kPenaltyThreads, smem, stream>>>(a, q);
+    SB_CUDA_CHECK(cudaGetLastError());
+  }
+  if (a.temperature > 0.f) {
+    // ln(min_p) on the host, in double, rounded once to fp32
+    const double min_p = std::min(a.min_p, 1.f);
+    const float log_min_p = a.min_p > 0.f ? static_cast<float>(std::log(min_p)) : 0.f;
+    sample_random_kernel<<<a.B, kSampleThreads, 0, stream>>>(a, log_min_p);
+  } else
     sample_greedy_kernel<<<a.B, kSampleThreads, 0, stream>>>(a);
   SB_CUDA_CHECK(cudaGetLastError());
   return 0;

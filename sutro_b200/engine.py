@@ -19,6 +19,7 @@ import torch
 from . import _lib as L
 from . import modelspec as MS
 from . import vocab as VB
+from .common import check_penalties
 from .schema_fsm import ByteDFA, FsmLimits, compile_schema, compile_thinking
 from .unicode_tables import class_table
 
@@ -62,7 +63,9 @@ class JobC(C.Structure):
                 ("out_first_logits_dev", C.c_void_p),
                 ("temperature", C.c_float), ("top_k", C.c_int), ("top_p", C.c_float),
                 ("seed", C.c_uint64), ("seed_per_row", C.c_int),
-                ("out_cum_logprob_dev", C.c_void_p), ("row_ids_dev", C.c_void_p)]
+                ("out_cum_logprob_dev", C.c_void_p), ("row_ids_dev", C.c_void_p),
+                ("presence_penalty", C.c_float), ("frequency_penalty", C.c_float),
+                ("repetition_penalty", C.c_float), ("min_p", C.c_float)]
 
 
 # indexed by SB200_KC_*; "rope" stays in the stats layout but counts 0: RoPE and the K/V write
@@ -126,7 +129,12 @@ class SampleArgsC(C.Structure):     # sb200_sample_args (test hook: one sampling
                 ("top_k", C.c_int), ("top_p", C.c_float), ("seed", C.c_uint64),
                 ("seed_per_row", C.c_int)] + \
                [(n, C.c_void_p) for n in ("row_ids", "slot_cum_logprob", "out_cum_logprob",
-                                          "out_tau")]
+                                          "out_tau")] + \
+               [(n, C.c_float) for n in ("presence_penalty", "frequency_penalty",
+                                         "repetition_penalty", "min_p")] + \
+               [("prompt_prefix", C.c_void_p), ("n_prompt_prefix", C.c_int),
+                ("prompt_suffix", C.c_void_p), ("n_prompt_suffix", C.c_int)] + \
+               [(n, C.c_void_p) for n in ("row_tokens", "row_tok_off", "slot_n_row_tok")]
 
 
 L.register("sb200_sample", C.c_int, [C.POINTER(SampleArgsC), C.c_void_p])
@@ -498,7 +506,8 @@ class LocalEngine:
 
     def _job_options(self, job: "JobC", system_prompt, json_schema, max_new_tokens, ignore_eos,
                      truncate_rows, share_prefix, fsm_limits, jump_forward, temperature, top_k,
-                     top_p, seed, seed_per_row, thinking_chars=None):
+                     top_p, seed, seed_per_row, thinking_chars=None, presence_penalty=0.0,
+                     frequency_penalty=0.0, repetition_penalty=1.0, min_p=0.0):
         """Fill the host-side fields of an sb200_job (prompt framing, schema automaton, jump-forward
         plan, sampling).  Returns (dfa, plan, keep) — `keep` holds the arrays the job points at."""
         emb_mode = self.spec.embedding_model
@@ -535,6 +544,8 @@ class LocalEngine:
                 job.fsm_tail_tok = _np_ptr(plan["tail_tok"], c_i32p)
         job.temperature, job.top_k, job.top_p = float(temperature), int(top_k), float(top_p)
         job.seed, job.seed_per_row = int(seed) & (2 ** 64 - 1), int(seed_per_row)
+        job.presence_penalty, job.frequency_penalty, job.repetition_penalty, job.min_p = \
+            check_penalties(presence_penalty, frequency_penalty, repetition_penalty, min_p)
         return dfa, plan, (pre, suf)
 
     def run_blob_dev(self, d_text: torch.Tensor, d_off: torch.Tensor, n_rows: int, n_bytes: int,
@@ -548,7 +559,9 @@ class LocalEngine:
                      temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0, seed: int = 0,
                      seed_per_row: bool = False, return_logprobs: bool = False,
                      row_ids: Optional[Sequence[int]] = None,
-                     thinking_chars: Optional[int] = None) -> Dict[str, Any]:
+                     thinking_chars: Optional[int] = None, presence_penalty: float = 0.0,
+                     frequency_penalty: float = 0.0, repetition_penalty: float = 1.0,
+                     min_p: float = 0.0) -> Dict[str, Any]:
         """Phase B of the hot path, HBM to HBM: a device-resident Arrow column (uint8 bytes +
         int64 offsets[n_rows+1]) -> tokenise -> prefill/decode (+mask) -> detokenise ->
         device-resident results (`d_bytes`/`d_boff`, `flat`/`ooff` tokens, `d_emb`, ...).
@@ -575,7 +588,8 @@ class LocalEngine:
             dfa, plan, keep = self._job_options(job, system_prompt, json_schema, max_new_tokens,
                                                 ignore_eos, truncate_rows, share_prefix, fsm_limits,
                                                 jump_forward, temperature, top_k, top_p, seed,
-                                                seed_per_row, thinking_chars)
+                                                seed_per_row, thinking_chars, presence_penalty,
+                                                frequency_penalty, repetition_penalty, min_p)
             job.row_tokens_dev, job.row_tok_off_dev = d_tok.data_ptr(), d_toff.data_ptr()
             job.row_tok_off, job.n_rows = _np_ptr(toff, c_i64p), n_rows
             job.out_tokens_dev = L.ptr(d_out)
@@ -668,7 +682,9 @@ class LocalEngine:
                  top_p: float = 1.0, seed: int = 0, seed_per_row: bool = False,
                  return_logprobs: bool = False,
                  row_ids: Optional[Sequence[int]] = None,
-                 thinking_chars: Optional[int] = None) -> GenerationResult:
+                 thinking_chars: Optional[int] = None, presence_penalty: float = 0.0,
+                 frequency_penalty: float = 0.0, repetition_penalty: float = 1.0,
+                 min_p: float = 0.0) -> GenerationResult:
         """The whole hot path for one frame column.  Three phases, timed separately:
           A  host -> HBM   : rows -> Arrow blob, template/schema compile (cached), H2D copy
           B  device        : tokenize, prefill/decode (+mask), detokenize — HBM to HBM
@@ -707,7 +723,10 @@ class LocalEngine:
                                   jump_forward=jump_forward, temperature=temperature, top_k=top_k,
                                   top_p=top_p, seed=seed, seed_per_row=seed_per_row,
                                   return_logprobs=return_logprobs, row_ids=row_ids,
-                                  thinking_chars=thinking_chars)
+                                  thinking_chars=thinking_chars,
+                                  presence_penalty=presence_penalty,
+                                  frequency_penalty=frequency_penalty,
+                                  repetition_penalty=repetition_penalty, min_p=min_p)
             t_b = time.perf_counter()
             # ---- phase C ---------------------------------------------------------
             outputs = out_tokens = emb = None
@@ -744,7 +763,9 @@ def _infer_one_call(self, rows, system_prompt: Optional[str] = None,
                     return_logprobs: bool = False, return_tokens: bool = True,
                     progress: Optional[Callable[[int, int, int], None]] = None,
                     profile: bool = False,
-                    thinking_chars: Optional[int] = None) -> GenerationResult:
+                    thinking_chars: Optional[int] = None, presence_penalty: float = 0.0,
+                    frequency_penalty: float = 0.0, repetition_penalty: float = 1.0,
+                    min_p: float = 0.0) -> GenerationResult:
     """The same job through `sb200_infer_text`: ONE C-ABI call with host buffers in and out
     (what a non-Python host would bind; the SDK's infer() and bench.py's `e2e` use it).
     `generate` is the phased form of the same work; the results are identical.  The call times
@@ -761,7 +782,8 @@ def _infer_one_call(self, rows, system_prompt: Optional[str] = None,
     dfa, plan, keep = self._job_options(job, system_prompt, json_schema, max_new_tokens,
                                         ignore_eos, truncate_rows, share_prefix, fsm_limits,
                                         jump_forward, temperature, top_k, top_p, seed, seed_per_row,
-                                        thinking_chars)
+                                        thinking_chars, presence_penalty, frequency_penalty,
+                                        repetition_penalty, min_p)
     cb = PROGRESS_FN(lambda r, i, o, u: progress(r, i, o)) if progress else PROGRESS_FN()
     job.progress = cb
     job.profile = int(profile)

@@ -30,7 +30,8 @@ from typing import Any, Dict, List, Optional, Type, Union
 import numpy as np
 import pandas as pd
 
-from .common import (ModelOptions, column_as_arrow, handle_data_helper, is_frame,
+from .common import (ModelOptions, check_penalties, column_as_arrow, handle_data_helper,
+                     is_frame,
                      normalize_output_schema, pl, to_colored_text)
 from .interfaces import BaseSutroClient, JobStatus
 from .templates import Templates
@@ -233,7 +234,8 @@ class Sutro(Templates, BaseSutroClient):
         # the local engine understands the usual keys and rejects the rest loudly.
         sp = dict(sampling_params or {})
         known = {"temperature", "top_p", "top_k", "seed", "random_seed", "max_tokens",
-                 "max_new_tokens", "ignore_eos", "max_thinking_chars"}
+                 "max_new_tokens", "ignore_eos", "max_thinking_chars", "presence_penalty",
+                 "frequency_penalty", "repetition_penalty", "min_p"}
         unknown = sorted(set(sp) - known)
         if unknown:
             raise ValueError(f"unsupported sampling_params for the local engine: {unknown} "
@@ -244,6 +246,12 @@ class Sutro(Templates, BaseSutroClient):
         if temperature < 0 or not (0.0 < top_p <= 1.0) or top_k < 0:
             raise ValueError("sampling_params: temperature >= 0, 0 < top_p <= 1, top_k >= 0")
         seed = int(sp.get("seed", sp.get("random_seed", 0)) or 0)
+        # vLLM's keys and ranges (None = the neutral value, as vLLM reads it)
+        penalties = dict(zip(
+            ("presence_penalty", "frequency_penalty", "repetition_penalty", "min_p"),
+            check_penalties(*(sp[k] if sp.get(k) is not None else d for k, d in (
+                ("presence_penalty", 0.0), ("frequency_penalty", 0.0),
+                ("repetition_penalty", 1.0), ("min_p", 0.0))))))
         max_new = sp.get("max_tokens", sp.get("max_new_tokens"))
         max_new = None if max_new is None else int(max_new)
 
@@ -285,6 +293,9 @@ class Sutro(Templates, BaseSutroClient):
                       truncate_rows=truncate_rows, temperature=temperature, top_k=top_k,
                       top_p=top_p, seed=seed, seed_per_row=bool(random_seed_per_input),
                       return_logprobs=True, progress=stream)
+            # only non-neutral values are passed: engines without them keep working
+            kw.update({k: v for k, v in penalties.items()
+                       if v != (1.0 if k == "repetition_penalty" else 0.0)})
             if thinking is not None:
                 kw["thinking_chars"] = thinking
             if self.fsm_limits is not None:

@@ -12,10 +12,12 @@
 // the G query heads of the kv head into 128 rows (row = token*G + head), so K/V are read once
 // per GQA group and the causal frontier advances in QT-token steps.  KV is consumed in blocks
 // of up to 128 tokens: first the prefix blocks, then the row's own blocks up to the tile's
-// diagonal.  Only the valid tokens (rounded up to 32-row TMA boxes) are loaded; the MMAs always
-// cover the whole 128-token block (a data-dependent wgmma count would make ptxas serialise
-// them), with P = 0 on the columns past the valid ones (selected, not multiplied, so garbage K
-// rows cannot leak into P).  0 * V stays 0 only where V is finite, so the CALLER must keep the
+// diagonal.  Only the valid tokens (rounded up to 32-row TMA boxes) are loaded, and the MMAs
+// cover the same 32, 64, 96 or 128 columns: each width is its own fully unrolled path (a
+// data-dependent wgmma count would make ptxas serialise them).  P = 0 on the columns past the
+// valid ones (selected, not multiplied, so garbage K rows cannot leak into P); the columns a
+// narrower block drops would only have added zero products.  0 * V stays 0 only where V is
+// finite, so the CALLER must keep the
 // k/v columns of the qkv buffer and the prefix buffer finite in every row a 32-row box can reach
 // past a sequence's last token (the engine zeroes both buffers when it allocates them).  Rows
 // past the loaded ones hold an earlier block's V or the zeros the V ring starts with.
@@ -220,79 +222,92 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
       int j0, n16;
       tc_block<G>(ge, b, is_pre, j0, n16);
       const uint32_t st = g & 1, par = (g >> 1) & 1;
-      // ---- S = Q K^T (64 x 128 per warpgroup) ----
-      float s[64];
-      mbar_wait(bar(K_FULL + st), par);
-      wgmma_fence();
+      // One block at MMA width W: the n16 valid columns rounded up to 32.  Each width is its own
+      // unrolled path (a data-dependent wgmma count would be serialised by ptxas).  Columns in
+      // [n16, W) are masked to P = 0 as before; the columns past W, which the full-width MMAs
+      // used to cover, would only have added zero products, so O and l are unchanged.
+      auto run_block = [&](auto width) {
+        constexpr int W = decltype(width)::value;
+        // ---- S = Q K^T (64 x W per warpgroup) ----
+        float s[W / 2];
+        mbar_wait(bar(K_FULL + st), par);
+        wgmma_fence();
 #pragma unroll
-      for (int dh = 0; dh < 2; ++dh)
+        for (int dh = 0; dh < 2; ++dh)
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          wgmma_m64n128k16_ss(s, gmma_desc_k_sw128(s_qw + dh * kHalfBytes + 32 * k),
-                              gmma_desc_k_sw128(s_k + st * kTileBytes2 + dh * kHalfBytes + 32 * k),
-                              (dh | k) != 0);
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(s);
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(bar(K_EMPTY + st));
-        if (b == ge.n_blocks - 1) mbar_arrive(bar(Q_EMPTY));
-      }
-      // ---- softmax: s[4j + 2h + e] is row h, column 8j + 2 q4 + e of the block ----
-      uint32_t pa[32];   // P as bf16x2: the A fragments of the eight K=16 steps of P.V
+          for (int k = 0; k < 4; ++k)
+            wgmma_ss_n(s, gmma_desc_k_sw128(s_qw + dh * kHalfBytes + 32 * k),
+                       gmma_desc_k_sw128(s_k + st * kTileBytes2 + dh * kHalfBytes + 32 * k),
+                       (dh | k) != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(s);
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(bar(K_EMPTY + st));
+          if (b == ge.n_blocks - 1) mbar_arrive(bar(Q_EMPTY));
+        }
+        // ---- softmax: s[4j + 2h + e] is row h, column 8j + 2 q4 + e of the block ----
+        uint32_t pa[W / 4];   // P as bf16x2: the A fragments of the W/16 K=16 steps of P.V
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        // columns c of this block are valid for this row iff c < vlim
-        const int vlim = min(is_pre ? ge.past - j0 : ge.qt0 + t_in[h] - j0 + 1, n16);
-        float mx = -INFINITY;
+        for (int h = 0; h < 2; ++h) {
+          // columns c of this block are valid for this row iff c < vlim
+          const int vlim = min(is_pre ? ge.past - j0 : ge.qt0 + t_in[h] - j0 + 1, n16);
+          float mx = -INFINITY;
 #pragma unroll
-        for (int j = 0; j < 16; ++j)
+          for (int j = 0; j < W / 8; ++j)
 #pragma unroll
-          for (int e = 0; e < 2; ++e)
-            if (8 * j + 2 * q4 + e < vlim) mx = fmaxf(mx, s[4 * j + 2 * h + e]);
-        mx = quad_max(mx) * scale_log2;   // scale > 0: max commutes with the scaling
-        if (b == 0) {
-          m_used[h] = (mx == -INFINITY) ? 0.f : mx;
-        } else if (mx > m_used[h] + kRescaleThreshold) {
-          const float alpha = ex2_approx(m_used[h] - mx);
-          m_used[h] = mx;
-          l_run[h] *= alpha;
+            for (int e = 0; e < 2; ++e)
+              if (8 * j + 2 * q4 + e < vlim) mx = fmaxf(mx, s[4 * j + 2 * h + e]);
+          mx = quad_max(mx) * scale_log2;   // scale > 0: max commutes with the scaling
+          if (b == 0) {
+            m_used[h] = (mx == -INFINITY) ? 0.f : mx;
+          } else if (mx > m_used[h] + kRescaleThreshold) {
+            const float alpha = ex2_approx(m_used[h] - mx);
+            m_used[h] = mx;
+            l_run[h] *= alpha;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            o[4 * j + 2 * h] *= alpha;
-            o[4 * j + 2 * h + 1] *= alpha;
+            for (int j = 0; j < 16; ++j) {
+              o[4 * j + 2 * h] *= alpha;
+              o[4 * j + 2 * h + 1] *= alpha;
+            }
           }
-        }
-        const float neg_m = -m_used[h];
-        float ps = 0.f;
+          const float neg_m = -m_used[h];
+          float ps = 0.f;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int c0 = 8 * j + 2 * q4;
-          float p0 = ex2_approx(fmaf(s[4 * j + 2 * h], scale_log2, neg_m));
-          float p1 = ex2_approx(fmaf(s[4 * j + 2 * h + 1], scale_log2, neg_m));
-          p0 = c0 < vlim ? p0 : 0.f;
-          p1 = c0 + 1 < vlim ? p1 : 0.f;
-          ps += p0 + p1;
-          // K step kk = j / 2: a0/a1 = rows 0/8 at k 2q4, a2/a3 = rows 0/8 at k 8 + 2q4
-          pa[4 * (j >> 1) + 2 * (j & 1) + h] = pack_bf16x2(p0, p1);
+          for (int j = 0; j < W / 8; ++j) {
+            const int c0 = 8 * j + 2 * q4;
+            float p0 = ex2_approx(fmaf(s[4 * j + 2 * h], scale_log2, neg_m));
+            float p1 = ex2_approx(fmaf(s[4 * j + 2 * h + 1], scale_log2, neg_m));
+            p0 = c0 < vlim ? p0 : 0.f;
+            p1 = c0 + 1 < vlim ? p1 : 0.f;
+            ps += p0 + p1;
+            // K step kk = j / 2: a0/a1 = rows 0/8 at k 2q4, a2/a3 = rows 0/8 at k 8 + 2q4
+            pa[4 * (j >> 1) + 2 * (j & 1) + h] = pack_bf16x2(p0, p1);
+          }
+          l_run[h] += ps;
         }
-        l_run[h] += ps;
-      }
-      // ---- O += P V ----
-      mbar_wait(bar(V_FULL + st), par);
-      wgmma_fence();
+        // ---- O += P V ----
+        mbar_wait(bar(V_FULL + st), par);
+        wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
-        const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
-        wgmma_m64n128k16_rs_tb(
-            o, a, gmma_desc_sw128(s_v + st * kTileBytes2 + kk * 2048, kHalfBytes, 1024));
+        for (int kk = 0; kk < W / 16; ++kk) {
+          const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+          wgmma_m64n128k16_rs_tb(
+              o, a, gmma_desc_sw128(s_v + st * kTileBytes2 + kk * 2048, kHalfBytes, 1024));
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar(V_EMPTY + st));
+      };
+      switch ((n16 - 1) >> 5) {  // n16 is in [16, 128]
+        case 0: run_block(std::integral_constant<int, 32>{}); break;
+        case 1: run_block(std::integral_constant<int, 64>{}); break;
+        case 2: run_block(std::integral_constant<int, 96>{}); break;
+        default: run_block(std::integral_constant<int, 128>{}); break;
       }
-      wgmma_commit();
-      wgmma_wait<0>();
-      wgmma_fence_regs(o);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar(V_EMPTY + st));
     }
     // ---- epilogue: O / l -> bf16 -> global ----
 #pragma unroll

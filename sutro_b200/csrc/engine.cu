@@ -207,6 +207,7 @@ static_assert(sizeof(SeqInit) % 4 == 0, "SeqInit records are staged as int32 wor
 struct PrefillStep {
   const int32_t* work;  // work items of the dense prefill attention
   int n_work;
+  int n_seqs;
   const int32_t *q_start, *q_len, *past;  // per sequence
   bool keep_prefix;  // this pass is the shared prefix's: keep its K/V in prefix_kv
 };
@@ -322,9 +323,28 @@ struct Engine {
     return gemm_bf16_tn(a, a_rows, wt, d, r, M, N, K, ldd, epi, 0, stream, qa);
   }
 
+  // O (+ residual), RMSNorm, gate/up (SwiGLU) and down (+ residual) of layer l over M rows:
+  // a [M, q_dim] and the residual stream in [M, d_model] rows of x_in -> x_out (may alias).
+  int layer_tail(int l, const bf16* a, int a_rows, bf16* x_in, bf16* x_out, int M) {
+    const auto& c = cfg;
+    SB_K(SB200_KC_GEMM, gemm(a, a_rows, wo[l], x_in, x_in, M, c.d_model, q_dim, c.d_model,
+                             EPI_RESIDUAL_BF16));
+    SB_K(SB200_KC_NORM, rmsnorm(x_in, ln2[l], h, M, c.d_model, c.rms_eps, stream));
+    SB_K(SB200_KC_GEMM, gemm(h, t_max, wgu[l], act, nullptr, M, 2 * c.d_ff, c.d_model, c.d_ff,
+                             EPI_SWIGLU_BF16));
+    SB_K(SB200_KC_GEMM, gemm(act, t_max, wd[l], x_out, x_in, M, c.d_model, c.d_ff, c.d_model,
+                             EPI_RESIDUAL_BF16));
+    return 0;
+  }
+
   // ---- one pass of the transformer stack over T flattened tokens -----------
   // prefill (pf != nullptr): attention over (cached prefix | new tokens) per sequence;
   // decode (pf == nullptr): one token per sequence against its paged history.
+  // Leaves the hidden state of the rows the head reads in rows [0, n) of x: decode's T rows,
+  // or each prefill sequence's last token.  Every layer's K/V covers all T tokens, but nothing
+  // reads the last layer's O/MLP output of a prefill token that is not its sequence's last, so
+  // that layer's tail runs on the last tokens only (rows do not depend on M: exact), and not
+  // at all in the shared prefix's pass, which has no head.
   int forward(int T, const PrefillStep* pf) {
     const auto& c = cfg;
     const float scale = 1.0f / sqrtf(static_cast<float>(kHeadDim));
@@ -355,28 +375,25 @@ struct Engine {
              attn_decode(qkv, attn, kv_layer(l), page_table, max_pages, row_slot, ctx_len, T,
                          c.n_q_heads, c.n_kv_heads, scale, stream));
       }
-      SB_K(SB200_KC_GEMM, gemm(attn, t_max, wo[l], x, x, T, c.d_model, q_dim, c.d_model,
-                               EPI_RESIDUAL_BF16));
-      SB_K(SB200_KC_NORM, rmsnorm(x, ln2[l], h, T, c.d_model, c.rms_eps, stream));
-      SB_K(SB200_KC_GEMM, gemm(h, t_max, wgu[l], act, nullptr, T, 2 * c.d_ff, c.d_model, c.d_ff,
-                               EPI_SWIGLU_BF16));
-      SB_K(SB200_KC_GEMM, gemm(act, t_max, wd[l], x, x, T, c.d_model, c.d_ff, c.d_model,
-                               EPI_RESIDUAL_BF16));
+      if (!pf || l + 1 < c.n_layers) {
+        if (layer_tail(l, attn, t_max, x, x, T)) return -1;
+      } else if (!pf->keep_prefix) {
+        // last tokens: attention rows -> the dead qkv buffer (wider than attn: they fit),
+        // residual rows -> hl; the down GEMM writes the result to rows [0, n) of x
+        const int n = pf->n_seqs;
+        SB_K(SB200_KC_EMBED, gather_rows(last_idx, attn, qkv, n, q_dim, stream));
+        SB_K(SB200_KC_EMBED, gather_rows(last_idx, x, hl, n, c.d_model, stream));
+        if (layer_tail(l, qkv, n, hl, x, n)) return -1;
+      }
     }
     return 0;
   }
 
-  // final norm + lm_head + masked greedy sampling for `n` rows whose hidden
-  // states are rows idx[0..n) of x (idx == nullptr: rows 0..n).
-  int head_and_sample(int n, const int32_t* idx, const int32_t* d_row_slot,
-                      const sb200_job& job, bool has_fsm, bool first_decision = false) {
+  // final norm + lm_head + masked greedy sampling for the `n` rows [0, n) of x
+  int head_and_sample(int n, const int32_t* d_row_slot, const sb200_job& job, bool has_fsm,
+                      bool first_decision = false) {
     const auto& c = cfg;
-    const bf16* src = x;
-    if (idx) {
-      SB_K(SB200_KC_EMBED, gather_rows(idx, x, hl, n, c.d_model, stream));
-      src = hl;
-    }
-    SB_K(SB200_KC_NORM, rmsnorm(src, w.final_norm, hn, n, c.d_model, c.rms_eps, stream));
+    SB_K(SB200_KC_NORM, rmsnorm(x, w.final_norm, hn, n, c.d_model, c.rms_eps, stream));
     const bool has_tails = has_fsm && job.fsm_tail_off != nullptr;
     for (int r0 = 0; r0 < n; r0 += logit_rows) {
       const int nr = std::min(logit_rows, n - r0);
@@ -711,19 +728,18 @@ struct JobRun {
           e.kv_pool, e.layer_stride, kv_page_elems(c.n_kv_heads), prefix_tail_page, d.copy);
     }
     SB_CUDA_CHECK(cudaGetLastError());
-    const PrefillStep step{d.work, n_work, d.q_start, d.q_len, d.past, prefix_pass};
+    const PrefillStep step{d.work, n_work, n, d.q_start, d.q_len, d.past, prefix_pass};
     if (e.forward(T, &step)) return -1;
     if (prefix_pass) return 0;
     if (p.embed_mode) {
-      if (gather_rows(e.last_idx, e.x, e.hl, n, c.d_model, e.stream)) return -1;
-      if (rmsnorm(e.hl, e.w.final_norm, e.hn, n, c.d_model, c.rms_eps, e.stream)) return -1;
+      if (rmsnorm(e.x, e.w.final_norm, e.hn, n, c.d_model, c.rms_eps, e.stream)) return -1;
       if (l2_normalize_rows(e.hn, e.embed_tmp, n, c.d_model, e.stream)) return -1;
       scatter_embed_kernel<<<n, 128, 0, e.stream>>>(e.embed_tmp, d.seqs, job.out_embed_dev,
                                                     c.d_model);
       SB_CUDA_CHECK(cudaGetLastError());
       return 0;
     }
-    return e.head_and_sample(n, e.last_idx, d.slot, job, p.has_fsm, true);
+    return e.head_and_sample(n, d.slot, job, p.has_fsm, true);
   }
 
   // One decode step: one token for every slot in the decode batch.
@@ -737,7 +753,7 @@ struct JobRun {
     const int prc = prepare_decode(e.row_slot, e.slot_next_tok, e.slot_pos, e.tok_ids, e.tok_pos,
                                    e.tok_slot, e.ctx_len, B, e.stream);
     e.prof.end();
-    if (prc || e.forward(B, nullptr) || e.head_and_sample(B, nullptr, e.row_slot, job, p.has_fsm))
+    if (prc || e.forward(B, nullptr) || e.head_and_sample(B, e.row_slot, job, p.has_fsm))
       return -1;
     decode_tokens += B;
     ++steps_decode;

@@ -15,6 +15,12 @@
 //     the G query heads as the (zero-padded) M rows; online softmax uses
 //     quad-level warp shuffles; the warp normalises and writes its output
 //     itself: no cross-warp merge and no block-wide barrier.
+//   * Split-KV for long rows: a row of more than kDecodeSplitTokens tokens is cut at absolute
+//     positions s * kDecodeSplitTokens into splits, one warp per (row, kv head, split).  Such a
+//     warp writes its unnormalised fp32 partial (O, running max, sum) to a workspace, and a
+//     merge kernel combines each row's splits in split order.  A row of at most
+//     kDecodeSplitTokens tokens is one split: its warp runs the single-warp path above and
+//     writes its output directly.  Either way a row's output depends on the row alone.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -130,13 +136,27 @@ SB_DEVICE void decode_tile(uint32_t ks, const uint32_t (&qa)[8][2], int tile, in
   }
 }
 
+// Partial of one (row, kv head, split) unit in the workspace: O[G][128], m[G], l[G] (fp32).
+SB_DEVICE float* unit_partial(float* ws, int i, int kvh, int split, int hkv, int max_splits,
+                              int G) {
+  return ws + (static_cast<size_t>(i * hkv + kvh) * max_splits + split) * G * (kHeadDim + 2);
+}
+
+SB_DEVICE int n_splits_of(int L) { return (L + kDecodeSplitTokens - 1) / kDecodeSplitTokens; }
+
+// Warps [0, n_split_units) are split units: unit u is (split row u / hkv / max_splits, kv head,
+// split); split row i is batch row split_rows[i] (or i when split_rows is null).  They come first
+// so that long rows start early.  The n_pairs warps after them are (row, kv head) pairs; a pair
+// whose row has more than one split leaves it to the split units when there are any.
 template <int G>
 __global__ void __launch_bounds__(kDecWarps * 32)
 attn_decode_warp_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ out,
                         const __nv_bfloat16* __restrict__ kv_layer,
                         const int32_t* __restrict__ page_table, int max_pages,
                         const int32_t* __restrict__ row_slot, const int32_t* __restrict__ ctx_len,
-                        int n_pairs, int hq, int hkv, float scale_log2) {
+                        int n_pairs, int hq, int hkv, float scale_log2,
+                        const int32_t* __restrict__ split_rows, int n_split_units, int max_splits,
+                        float* __restrict__ ws) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~static_cast<uintptr_t>(127));
@@ -144,21 +164,39 @@ attn_decode_warp_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int pair = blockIdx.x * kDecWarps + warp;
-  if (pair >= n_pairs) return;  // whole warp exits together; no block-wide barriers below
-  const int b = pair / hkv;
-  const int kvh = pair - b * hkv;
+  int pair = blockIdx.x * kDecWarps + warp;
+  int b, kvh, split = 0, si = 0;
+  const bool split_unit = pair < n_split_units;
+  if (split_unit) {
+    const int e = pair / hkv;
+    kvh = pair - e * hkv;
+    si = e / max_splits;
+    split = e - si * max_splits;
+    b = split_rows != nullptr ? split_rows[si] : si;
+  } else {
+    pair -= n_split_units;
+    if (pair >= n_pairs) return;  // whole warp exits together; no block-wide barriers below
+    b = pair / hkv;
+    kvh = pair - b * hkv;
+  }
   const int slot = row_slot[b];
   const int L = ctx_len[b];
+  const int n_splits = n_splits_of(L);
+  if (split_unit ? (n_splits == 1 || split >= n_splits) : (n_splits > 1 && n_split_units > 0))
+    return;
   const int n_tiles = (L + kPageTokens - 1) / kPageTokens;
-  const int32_t* pt = page_table + static_cast<size_t>(slot) * max_pages;
+  // this warp's tiles: [t0, t1); a pair takes the whole row
+  const int t0 = split_unit ? split * (kDecodeSplitTokens / kPageTokens) : 0;
+  const int t1 = split_unit ? min(n_tiles, t0 + kDecodeSplitTokens / kPageTokens) : n_tiles;
+  const int n_mine = t1 - t0;
+  const int32_t* pt = page_table + static_cast<size_t>(slot) * max_pages + t0;
 
   uint8_t* my_smem = smem + warp * kDecStages * kStageBytes;
   ring_init(full_bar[warp], lane);
   if (lane == 0) {
 #pragma unroll
     for (int s = 0; s < kDecStages; ++s)
-      if (s < n_tiles) issue_page(kv_layer, pt[s], hkv, kvh, my_smem, full_bar[warp], s);
+      if (s < n_mine) issue_page(kv_layer, pt[s], hkv, kvh, my_smem, full_bar[warp], s);
   }
 
   const int qr = lane >> 2;
@@ -170,34 +208,86 @@ attn_decode_warp_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __
   for (int i = 0; i < 16; ++i) o[i][0] = o[i][1] = 0.f;
   float m_run = -INFINITY, l_run = 0.f;
 
-  for (int tile = 0; tile < n_tiles; ++tile) {
-    const int stage = tile % kDecStages;
-    const uint32_t phase = (tile / kDecStages) & 1;
+  for (int j = 0; j < n_mine; ++j) {
+    const int stage = j % kDecStages;
+    const uint32_t phase = (j / kDecStages) & 1;
     mbar_wait(smem_u32(&full_bar[warp][stage]), phase);
-    decode_tile(smem_u32(my_smem + stage * kStageBytes), qa, tile, L, scale_log2, lane, o, m_run,
-                l_run);
+    decode_tile(smem_u32(my_smem + stage * kStageBytes), qa, t0 + j, L, scale_log2, lane, o,
+                m_run, l_run);
     __syncwarp();
-    const int next = tile + kDecStages;
-    if (lane == 0 && next < n_tiles) {
+    const int next = j + kDecStages;
+    if (lane == 0 && next < n_mine) {
       fence_proxy_async_smem();  // generic-proxy reads above vs async-proxy write below
       issue_page(kv_layer, pt[next], hkv, kvh, my_smem, full_bar[warp], stage);
     }
   }
-  if (qr < G) {
-    const float inv = 1.0f / l_run;
-    __nv_bfloat16* op = out + static_cast<size_t>(b) * hq * kHeadDim + (kvh * G + qr) * kHeadDim +
-                        2 * (lane & 3);
+  if (qr >= G) return;
+  if (split_unit) {  // unnormalised partial; the merge kernel finishes the row
+    float* u = unit_partial(ws, si, kvh, split, hkv, max_splits, G);
+    float* op = u + qr * kHeadDim + 2 * (lane & 3);
 #pragma unroll
     for (int nt = 0; nt < 16; ++nt)
-      *reinterpret_cast<__nv_bfloat162*>(op + nt * 8) =
-          __floats2bfloat162_rn(o[nt][0] * inv, o[nt][1] * inv);
+      *reinterpret_cast<float2*>(op + nt * 8) = make_float2(o[nt][0], o[nt][1]);
+    if ((lane & 3) == 0) {
+      u[G * kHeadDim + qr] = m_run;
+      u[G * kHeadDim + G + qr] = l_run;
+    }
+    return;
   }
+  const float inv = 1.0f / l_run;
+  __nv_bfloat16* op = out + static_cast<size_t>(b) * hq * kHeadDim + (kvh * G + qr) * kHeadDim +
+                      2 * (lane & 3);
+#pragma unroll
+  for (int nt = 0; nt < 16; ++nt)
+    *reinterpret_cast<__nv_bfloat162*>(op + nt * 8) =
+        __floats2bfloat162_rn(o[nt][0] * inv, o[nt][1] * inv);
+}
+
+// One warp per (split row, query head): combines the row's splits in split order,
+//   M = max_s m_s,  w_s = 2^((m_s - M) * scale_log2),  out = bf16(sum_s w_s O_s / sum_s w_s l_s),
+// each lane owning 4 of the 128 dims.  Rows of one split were written by the decode kernel.
+__global__ void __launch_bounds__(128)
+attn_decode_merge_kernel(__nv_bfloat16* __restrict__ out, const int32_t* __restrict__ ctx_len,
+                         const int32_t* __restrict__ split_rows, int n_split_rows, int max_splits,
+                         int hq, int hkv, float scale_log2, const float* __restrict__ ws) {
+  const int w = blockIdx.x * 4 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (w >= n_split_rows * hq) return;
+  const int si = w / hq;
+  const int h = w - si * hq;
+  const int b = split_rows != nullptr ? split_rows[si] : si;
+  const int n = min(n_splits_of(ctx_len[b]), max_splits);
+  if (n <= 1) return;
+  const int G = hq / hkv;
+  const int kvh = h / G, g = h - kvh * G;
+  const size_t unit = static_cast<size_t>(G) * (kHeadDim + 2);
+  const float* u0 = ws + static_cast<size_t>(si * hkv + kvh) * max_splits * unit;
+  float m = -INFINITY;
+  for (int s = 0; s < n; ++s) m = fmaxf(m, u0[s * unit + G * kHeadDim + g]);
+  float l = 0.f, o[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int s = 0; s < n; ++s) {
+    const float* u = u0 + s * unit;
+    const float ws_s = exp2f((u[G * kHeadDim + g] - m) * scale_log2);
+    l = fmaf(u[G * kHeadDim + G + g], ws_s, l);
+    const float2 a = *reinterpret_cast<const float2*>(u + g * kHeadDim + 4 * lane);
+    const float2 c = *reinterpret_cast<const float2*>(u + g * kHeadDim + 4 * lane + 2);
+    o[0] = fmaf(a.x, ws_s, o[0]);
+    o[1] = fmaf(a.y, ws_s, o[1]);
+    o[2] = fmaf(c.x, ws_s, o[2]);
+    o[3] = fmaf(c.y, ws_s, o[3]);
+  }
+  const float inv = 1.0f / l;
+  __nv_bfloat162* op = reinterpret_cast<__nv_bfloat162*>(
+      out + static_cast<size_t>(b) * hq * kHeadDim + h * kHeadDim + 4 * lane);
+  op[0] = __floats2bfloat162_rn(o[0] * inv, o[1] * inv);
+  op[1] = __floats2bfloat162_rn(o[2] * inv, o[3] * inv);
 }
 
 template <int G>
 int launch(const void* qkv, void* out, const void* kv_layer, const int32_t* page_table,
            int max_pages, const int32_t* row_slot, const int32_t* ctx_len, int B, int hq, int hkv,
-           float scale, cudaStream_t stream) {
+           float scale, const int32_t* split_rows, int n_split_rows, int max_splits, float* ws,
+           cudaStream_t stream) {
   auto* q = static_cast<const __nv_bfloat16*>(qkv);
   auto* o = static_cast<__nv_bfloat16*>(out);
   auto* kv = static_cast<const __nv_bfloat16*>(kv_layer);
@@ -206,10 +296,18 @@ int launch(const void* qkv, void* out, const void* kv_layer, const int32_t* page
   // tokens depend on its neighbours.
   auto kern = attn_decode_warp_kernel<G>;
   SB_SET_MAX_SMEM(kern, kDecSmem);
-  const int n_pairs = B * hkv;
-  kern<<<(n_pairs + kDecWarps - 1) / kDecWarps, kDecWarps * 32, kDecSmem, stream>>>(
-      q, o, kv, page_table, max_pages, row_slot, ctx_len, n_pairs, hq, hkv, scale_log2);
+  const bool split = max_splits > 1 && n_split_rows > 0;
+  const int n_split_units = split ? n_split_rows * hkv * max_splits : 0;
+  const int n_warps = n_split_units + B * hkv;
+  kern<<<(n_warps + kDecWarps - 1) / kDecWarps, kDecWarps * 32, kDecSmem, stream>>>(
+      q, o, kv, page_table, max_pages, row_slot, ctx_len, B * hkv, hq, hkv, scale_log2,
+      split_rows, n_split_units, max_splits, ws);
   SB_CUDA_CHECK(cudaGetLastError());
+  if (split) {
+    attn_decode_merge_kernel<<<(n_split_rows * hq + 3) / 4, 128, 0, stream>>>(
+        o, ctx_len, split_rows, n_split_rows, max_splits, hq, hkv, scale_log2, ws);
+    SB_CUDA_CHECK(cudaGetLastError());
+  }
   return 0;
 }
 
@@ -217,11 +315,12 @@ int launch(const void* qkv, void* out, const void* kv_layer, const int32_t* page
 
 int attn_decode(const void* qkv, void* out, const void* kv_layer, const int32_t* page_table,
                 int max_pages, const int32_t* row_slot, const int32_t* ctx_len, int B, int hq,
-                int hkv, float scale, cudaStream_t stream) {
+                int hkv, float scale, const int32_t* split_rows, int n_split_rows, int max_splits,
+                float* ws, cudaStream_t stream) {
   if (B <= 0) return 0;
   return dispatch_gqa("attn_decode", hq, hkv, [&](auto g) {
     return launch<g.value>(qkv, out, kv_layer, page_table, max_pages, row_slot, ctx_len, B, hq,
-                           hkv, scale, stream);
+                           hkv, scale, split_rows, n_split_rows, max_splits, ws, stream);
   });
 }
 

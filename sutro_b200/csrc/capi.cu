@@ -90,8 +90,20 @@ int sb200_rope_kv_write(void* qkv, const void* q_norm_w, const void* k_norm_w, c
 int sb200_attn_decode(const void* qkv, void* out, const void* kv_layer, const int32_t* page_table,
                       int max_pages, const int32_t* row_slot, const int32_t* ctx_len, int B, int hq,
                       int hkv, float scale, void* stream) {
-  return attn_decode(qkv, out, kv_layer, page_table, max_pages, row_slot, ctx_len, B, hq, hkv,
-                     scale, STREAM(stream));
+  // The contexts live on the device; max_pages bounds them without a synchronise.  A bound
+  // past kDecodeSplitTokens lets every row split, in a workspace allocated stream-ordered.
+  const int max_splits = attn_decode_splits(static_cast<int64_t>(max_pages) * kPageTokens);
+  if (max_splits <= 1 || B <= 0)
+    return attn_decode(qkv, out, kv_layer, page_table, max_pages, row_slot, ctx_len, B, hq, hkv,
+                       scale, nullptr, 0, 1, nullptr, STREAM(stream));
+  float* ws = nullptr;
+  SB_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&ws),
+                                attn_decode_ws_floats(B, hq, max_splits) * sizeof(float),
+                                STREAM(stream)));
+  const int rc = attn_decode(qkv, out, kv_layer, page_table, max_pages, row_slot, ctx_len, B, hq,
+                             hkv, scale, nullptr, B, max_splits, ws, STREAM(stream));
+  SB_CUDA_CHECK(cudaFreeAsync(ws, STREAM(stream)));
+  return rc;
 }
 
 // Kept for callers of ABI version 1 (see the header).

@@ -10,7 +10,8 @@
 // Memory plan (see DESIGN.md): weights are caller-owned device tensors; the
 // engine owns the KV pool (num_pages x layers x hkv x 8 KiB), activation
 // workspaces sized for max(max_prefill_tokens, max_slots) tokens, a logits
-// chunk, the page table and the per-slot decode state.
+// chunk, the page table and the per-slot decode state; the split-KV decode
+// workspace grows with the longest rows a decode step has seen.
 #include <algorithm>
 #include <string>
 #include <utility>
@@ -62,16 +63,17 @@ prefill_prepare_kernel(const SeqInit* __restrict__ seqs, const int32_t* __restri
 // Install page-table rows and decode state for newly admitted rows.
 __global__ void __launch_bounds__(128)
 init_slots_kernel(const SeqInit* __restrict__ seqs, const int32_t* __restrict__ pt_rows,
-                  int max_pages, int32_t* __restrict__ page_table, int32_t* slot_state,
-                  int32_t* slot_ngen, int32_t* slot_pos, int32_t* slot_done, int32_t* slot_row,
-                  int32_t* slot_maxnew, int32_t* slot_next_tok, const int32_t* __restrict__ forced,
+                  int pt_cols, int max_pages, int32_t* __restrict__ page_table,
+                  int32_t* slot_state, int32_t* slot_ngen, int32_t* slot_pos, int32_t* slot_done,
+                  int32_t* slot_row, int32_t* slot_maxnew, int32_t* slot_next_tok, const int32_t* __restrict__ forced,
                   int n_forced, int32_t* __restrict__ out_tokens, int32_t* __restrict__ out_len,
                   int out_stride, float* __restrict__ slot_cum_logprob,
                   int32_t* __restrict__ slot_n_row_tok) {
   const SeqInit s = seqs[blockIdx.x];
-  for (int i = threadIdx.x; i < max_pages; i += blockDim.x)
+  // the first pt_cols entries: every page the row reserved; nothing reads the entries past them
+  for (int i = threadIdx.x; i < pt_cols; i += blockDim.x)
     page_table[static_cast<size_t>(s.slot) * max_pages + i] =
-        pt_rows[static_cast<size_t>(blockIdx.x) * max_pages + i];
+        pt_rows[static_cast<size_t>(blockIdx.x) * pt_cols + i];
   // jump-forward: the forced output prefix was fed with the prompt; it is output too
   if (s.row >= 0 && out_tokens != nullptr)
     for (int i = threadIdx.x; i < n_forced; i += blockDim.x)
@@ -180,16 +182,16 @@ __global__ void scatter_logits_kernel(const float* __restrict__ logits,
 struct StageLayout {
   struct View {     // the sections of one buffer, host or device
     SeqInit* seqs;  // [n_seqs]
-    int32_t* pt;    // [n_seqs][max_pages] page-table rows
+    int32_t* pt;    // [n_seqs][pt_cols] page-table rows: the pages the rows reserved
     int32_t* work;  // [n_work][2] {sequence, first query token}: dense prefill attention items
     int32_t *slot, *q_start, *q_len, *past;  // [n_seqs] each: that attention's sequence arrays
     int32_t* copy;  // [n_seqs] page to seed with the shared prefix's partial last page, or -1
   };
   size_t pt, work, slot, q_start, q_len, past, copy, words;  // offsets, and the total
 
-  StageLayout(size_t n_seqs, size_t n_work, size_t max_pages)
+  StageLayout(size_t n_seqs, size_t n_work, size_t pt_cols)
       : pt(n_seqs * (sizeof(SeqInit) / 4)),
-        work(pt + n_seqs * max_pages),
+        work(pt + n_seqs * pt_cols),
         slot(work + 2 * n_work),
         q_start(slot + n_seqs),
         q_len(q_start + n_seqs),
@@ -212,6 +214,13 @@ struct PrefillStep {
   bool keep_prefix;  // this pass is the shared prefix's: keep its K/V in prefix_kv
 };
 
+// What forward() needs of a decode step whose rows may exceed kDecodeSplitTokens: the batch rows
+// that may (device), and the most splits any of them has.  n_rows == 0: no row is split.
+struct DecodeSplit {
+  const int32_t* rows;
+  int n_rows, max_splits;
+};
+
 }  // namespace
 
 struct Engine {
@@ -229,6 +238,8 @@ struct Engine {
   DevArray<int32_t> slot_state, slot_ngen, slot_next_tok, slot_pos, slot_done, slot_row,
       slot_maxnew, slot_n_row_tok;
   DevArray<float> slot_cum_logprob;
+  DevArray<int32_t> split_rows;  // a decode step's rows longer than kDecodeSplitTokens
+  DevArray<float> split_ws;      // their split-KV partials (attn_decode_ws_floats), grow-only
   // Staging: a prefill step's StageLayout, or a decode step's row_slot.  The host buffer is
   // written only after the stream has been synchronised since its previous copy was enqueued:
   // every step that copies it is followed by a synchronise (JobRun::retire, or the one after
@@ -288,7 +299,7 @@ struct Engine {
         page_table.alloc(S * max_pages) || slot_state.alloc(S) || slot_ngen.alloc(S) ||
         slot_next_tok.alloc(S) || slot_pos.alloc(S) || slot_done.alloc(S) ||
         slot_row.alloc(S) || slot_maxnew.alloc(S) || slot_cum_logprob.alloc(S) ||
-        slot_n_row_tok.alloc(S))
+        slot_n_row_tok.alloc(S) || split_rows.alloc(S))
       return -1;
     if (c.embedding_model) {
       if (embed_tmp.alloc(static_cast<size_t>(c.max_slots) * c.d_model)) return -1;
@@ -345,7 +356,7 @@ struct Engine {
   // reads the last layer's O/MLP output of a prefill token that is not its sequence's last, so
   // that layer's tail runs on the last tokens only (rows do not depend on M: exact), and not
   // at all in the shared prefix's pass, which has no head.
-  int forward(int T, const PrefillStep* pf) {
+  int forward(int T, const PrefillStep* pf, const DecodeSplit& ds = DecodeSplit{nullptr, 0, 1}) {
     const auto& c = cfg;
     const float scale = 1.0f / sqrtf(static_cast<float>(kHeadDim));
     SB_K(SB200_KC_EMBED, embed_gather(tok_ids, w.embed, x, T, c.d_model, stream));
@@ -373,7 +384,9 @@ struct Engine {
       } else {
         SB_K(SB200_KC_ATTN_DECODE,
              attn_decode(qkv, attn, kv_layer(l), page_table, max_pages, row_slot, ctx_len, T,
-                         c.n_q_heads, c.n_kv_heads, scale, stream));
+                         c.n_q_heads, c.n_kv_heads, scale, ds.rows, ds.n_rows, ds.max_splits,
+                         split_ws, stream));
+        if (ds.n_rows > 0) ++prof.launches[SB200_KC_ATTN_DECODE];  // the split merge
       }
       if (!pf || l + 1 < c.n_layers) {
         if (layer_tail(l, attn, t_max, x, x, T)) return -1;
@@ -685,16 +698,20 @@ struct JobRun {
   int prefill(int T, bool prefix_pass) {
     const auto& c = e.cfg;
     const int n = static_cast<int>(batch.size());
-    int n_work = 0;
-    for (const SeqInit& s : batch) n_work += (s.q_len + e.q_tile - 1) / e.q_tile;
-    const StageLayout L(n, n_work, e.max_pages);
+    int n_work = 0, pt_cols = 1;
+    for (const SeqInit& s : batch) {
+      n_work += (s.q_len + e.q_tile - 1) / e.q_tile;
+      const int reserved = s.past / kPageTokens + static_cast<int>(slot_pages[s.slot].size());
+      pt_cols = std::max(pt_cols, reserved);
+    }
+    const StageLayout L(n, n_work, pt_cols);
     const StageLayout::View h = L.at(e.h_stage), d = L.at(e.d_stage);
     for (int i = 0, wi = 0; i < n; ++i) {
       const SeqInit& s = batch[i];
       const std::vector<int32_t>& own = slot_pages[s.slot];
       const int shared = s.past / kPageTokens;  // full prefix pages before the first own page
-      int32_t* pt = h.pt + static_cast<size_t>(i) * e.max_pages;
-      std::fill(pt, pt + e.max_pages, 0);
+      int32_t* pt = h.pt + static_cast<size_t>(i) * pt_cols;
+      std::fill(pt, pt + pt_cols, 0);
       std::copy(slot_pages[S].begin(), slot_pages[S].begin() + shared, pt);
       std::copy(own.begin(), own.end(), pt + shared);
       h.seqs[i] = s;
@@ -713,7 +730,7 @@ struct JobRun {
                                   e.stream));
     e.prof.launches[SB200_KC_OTHER] += 2;
     init_slots_kernel<<<n, 128, 0, e.stream>>>(
-        d.seqs, d.pt, e.max_pages, e.page_table, e.slot_state, e.slot_ngen, e.slot_pos,
+        d.seqs, d.pt, pt_cols, e.max_pages, e.page_table, e.slot_state, e.slot_ngen, e.slot_pos,
         e.slot_done, e.slot_row, e.slot_maxnew, e.slot_next_tok,
         e.d_suffix + (p.n_suffix - p.n_forced), p.n_forced,
         p.embed_mode ? nullptr : job.out_tokens_dev, p.embed_mode ? nullptr : job.out_len_dev,
@@ -753,7 +770,23 @@ struct JobRun {
     const int prc = prepare_decode(e.row_slot, e.slot_next_tok, e.slot_pos, e.tok_ids, e.tok_pos,
                                    e.tok_slot, e.ctx_len, B, e.stream);
     e.prof.end();
-    if (prc || e.forward(B, nullptr) || e.head_and_sample(B, e.row_slot, job, p.has_fsm))
+    // slot_ctx + 1 is each row's context in this step (prepare_decode: ctx = pos + 1)
+    int32_t* h_split = e.h_stage + B;
+    DecodeSplit ds{e.split_rows, 0, 1};
+    for (int b = 0; b < B; ++b) {
+      const int splits = attn_decode_splits(slot_ctx[active[b]] + 1);
+      if (splits > 1) {
+        h_split[ds.n_rows++] = b;
+        ds.max_splits = std::max(ds.max_splits, splits);
+      }
+    }
+    if (ds.n_rows > 0) {
+      if (e.split_ws.reserve(attn_decode_ws_floats(ds.n_rows, c.n_q_heads, ds.max_splits)))
+        return -1;
+      SB_CUDA_CHECK(cudaMemcpyAsync(e.split_rows, h_split, ds.n_rows * 4ull,
+                                    cudaMemcpyHostToDevice, e.stream));
+    }
+    if (prc || e.forward(B, nullptr, ds) || e.head_and_sample(B, e.row_slot, job, p.has_fsm))
       return -1;
     decode_tokens += B;
     ++steps_decode;

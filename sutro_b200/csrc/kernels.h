@@ -92,9 +92,23 @@ int rope_kv_write(void* qkv, const void* q_norm_w, const void* k_norm_w, const v
                   int hkv, float eps, cudaStream_t stream);
 
 // K2 — paged-KV decode attention (one query token per sequence).
+// A row of more than kDecodeSplitTokens tokens is attended in splits of kDecodeSplitTokens
+// tokens at absolute positions, merged in split order (split-KV); a shorter row is one split.
+// Rows split_rows[0 .. n_split_rows) (null: rows 0 .. n_split_rows) may be split, into at most
+// max_splits splits each; ws holds attn_decode_ws_floats() floats.  Every row longer than
+// kDecodeSplitTokens must be among them, unless max_splits <= 1 or n_split_rows == 0: then no
+// row is split, and the launch is the single-split kernel alone.
+constexpr int kDecodeSplitTokens = 4096;
+inline int attn_decode_splits(int64_t ctx) {
+  return static_cast<int>((ctx + kDecodeSplitTokens - 1) / kDecodeSplitTokens);
+}
+inline size_t attn_decode_ws_floats(int n_split_rows, int hq, int max_splits) {
+  return static_cast<size_t>(n_split_rows) * hq * max_splits * (kHeadDim + 2);
+}
 int attn_decode(const void* qkv, void* out, const void* kv_layer, const int32_t* page_table,
                 int max_pages, const int32_t* row_slot, const int32_t* ctx_len, int B, int hq,
-                int hkv, float scale, cudaStream_t stream);
+                int hkv, float scale, const int32_t* split_rows, int n_split_rows, int max_splits,
+                float* ws, cudaStream_t stream);
 
 // K3 — causal prefill attention over DENSE K/V: new tokens' K/V are the k/v columns
 // of the qkv buffer itself (post-norm/RoPE, written by the fused QKV epilogue), the shared

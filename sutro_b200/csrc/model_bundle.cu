@@ -263,7 +263,8 @@ int sb200_model_open(const char* dir, int device, int max_slots, int max_prefill
     c.embedding_model = static_cast<int>(num(*spec, "embedding_model"));
     c.eos_id = static_cast<int>(num(*spec, "eos_id"));
     c.max_slots = max_slots > 0 ? max_slots : 512;
-    c.max_prefill_tokens = max_prefill_tokens > 0 ? max_prefill_tokens : 8192;
+    // a prompt is never split over prefill steps: the default step holds one full-window row
+    c.max_prefill_tokens = max_prefill_tokens > 0 ? max_prefill_tokens : std::max(8192, c.max_position);
     c.logit_chunk_rows = 1024;
     c.min_admit_rows = std::max(1, c.max_slots / 4);
     for (auto& kv : spc->o) m->specials[kv.first] = static_cast<int>(strtod(kv.second.s.c_str(), nullptr));
@@ -409,7 +410,7 @@ int sb200_model_infer(void* model, const char* system_prompt_utf8, const char* j
     sb200_schema_tables(schema, &trans, &accept, &fin, &n_states, &start);
   }
   if (max_new_tokens <= 0) {  // the SDK's default budget (sdk.py _default_max_new_tokens)
-    const int cap = std::max(16, m->cfg.max_position / 2);
+    const int cap = std::max(16, std::min(m->cfg.max_position, 4096) / 2);
     const int64_t longest = constrained ? sb200_schema_longest_path(schema) : -1;
     max_new_tokens = longest >= 0 ? static_cast<int>(std::min<int64_t>(std::max<int64_t>(longest, 8), cap))
                                   : std::min(512, cap);

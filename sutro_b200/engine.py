@@ -369,10 +369,16 @@ class GenerationResult:
     cum_logprobs: Optional[np.ndarray] = None  # fp32 [n_rows] when return_logprobs=True
 
 
+def default_max_prefill_tokens(spec: MS.ModelSpec) -> int:
+    """A prompt is never split over prefill steps, so the default step holds one row that fills
+    the context window, and at least 8,192 tokens."""
+    return max(8192, spec.max_position)
+
+
 class LocalEngine:
     def __init__(self, spec: MS.ModelSpec, weights: MS.EngineWeights, vocab: VB.Vocab,
                  device: int | str | torch.device = 0, max_slots: int = 512,
-                 max_prefill_tokens: int = 8192, kv_pages: Optional[int] = None,
+                 max_prefill_tokens: Optional[int] = None, kv_pages: Optional[int] = None,
                  kv_fraction: float = 0.8, logit_chunk_rows: int = 1024,
                  min_admit_rows: Optional[int] = None):
         if not torch.cuda.is_available():
@@ -381,6 +387,8 @@ class LocalEngine:
         self.spec, self.weights, self.vocab = spec, weights, vocab
         if vocab.vocab_size != spec.vocab_size:
             raise ValueError("vocabulary size does not match the model")
+        if max_prefill_tokens is None:
+            max_prefill_tokens = default_max_prefill_tokens(spec)
         self.max_slots, self.max_prefill_tokens = max_slots, max_prefill_tokens
         with torch.cuda.device(self.device):
             self.cos, self.sin = (t.to(self.device).contiguous() for t in MS.rope_tables(spec))

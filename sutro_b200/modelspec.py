@@ -82,13 +82,17 @@ def _reg(s: ModelSpec) -> ModelSpec:
     return s
 
 
+# The real models serve 32,768-token windows: Qwen3's trained context, and for Llama-3.1 the
+# longest row one prefill step holds (a prompt is never split over prefill steps).
+CONTEXT_WINDOW = 32768
 QWEN3_0_6B = _reg(ModelSpec("qwen-3-0.6b", "qwen3", 28, 1024, 16, 8, 3072, 151936, True, 1e-6,
-                            1e6, True))
+                            1e6, True, max_position=CONTEXT_WINDOW))
 QWEN3_EMB_0_6B = _reg(replace(QWEN3_0_6B, name="qwen-3-embedding-0.6b", embedding_model=True))
 QWEN3_4B = _reg(ModelSpec("qwen-3-4b", "qwen3", 36, 2560, 32, 8, 9728, 151936, True, 1e-6, 1e6,
-                          True))
+                          True, max_position=CONTEXT_WINDOW))
 LLAMA31_8B = _reg(ModelSpec("llama-3.1-8b", "llama", 32, 4096, 32, 8, 14336, 128256, False, 1e-5,
-                            5e5, False, rope_scaling=_LLAMA31_SCALING))
+                            5e5, False, max_position=CONTEXT_WINDOW,
+                            rope_scaling=_LLAMA31_SCALING))
 # BASELINE.json says "llama-3-8b"; the reference's ModelOptions lists llama-3.1-8b
 # (sutro/common.py:22).  Same shapes; alias it.
 SPECS["llama-3-8b"] = LLAMA31_8B

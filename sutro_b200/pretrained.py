@@ -152,7 +152,7 @@ def _pretokenizer_digits(pre: Optional[Dict[str, Any]], path: str) -> Optional[i
 
 
 # --------------------------------------------------------------------------- config.json
-def spec_from_hf_config(cfg: Dict[str, Any], name: str, max_position: int = 4096,
+def spec_from_hf_config(cfg: Dict[str, Any], name: str, max_position: int = MS.CONTEXT_WINDOW,
                         embedding_model: bool = False) -> MS.ModelSpec:
     mt = cfg.get("model_type")
     if mt not in ("qwen3", "llama"):
@@ -211,7 +211,8 @@ def load_hf_weights(model_dir: str) -> Dict[str, "Any"]:
 
 
 def load_pretrained(model_dir: str, device=0, name: Optional[str] = None,
-                    max_position: int = 4096, embedding_model: Optional[bool] = None, **engine_kw):
+                    max_position: int = MS.CONTEXT_WINDOW, embedding_model: Optional[bool] = None,
+                    **engine_kw):
     """-> LocalEngine serving the checkpoint in `model_dir`."""
     from .engine import LocalEngine
     with open(os.path.join(model_dir, "config.json")) as f:

@@ -172,7 +172,9 @@ class Sutro(Templates, BaseSutroClient):
         schema's automaton accepts (every token is at least one byte), so a constrained row
         can always close its object — a row cut mid-object would not be JSON.  Free text: 512."""
         spec = getattr(eng, "spec", None)
-        cap = max(16, getattr(spec, "max_position", 4096) // 2)
+        # half the window, but no more than 2,048 tokens: a job's default budget does not grow
+        # with the context window
+        cap = max(16, min(getattr(spec, "max_position", 4096), 4096) // 2)
         if thinking_chars is not None and hasattr(eng, "compile_schema"):
             longest = eng.compile_schema(json_schema, limits, int(thinking_chars)).longest_path()
             return int(min(max(longest, 8), cap)) if longest is not None else \

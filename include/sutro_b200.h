@@ -120,10 +120,10 @@ int sb200_fsm_build_mask(const int32_t* fsm_trans, const uint8_t* fsm_accept, in
 /* Test hook: one sampling step (K8) exactly as the engine runs it on a chunk of logits rows:
  * the penalty kernel when a penalty is active (it rewrites `logits` in place), then the greedy or
  * the stochastic kernel.
- * The fields mirror the engine's internal arguments one for one; every pointer is a device
- * pointer.  Values are used as given: temperature <= 0 runs the greedy kernel (arg-max, lowest
- * index wins ties), top_k <= 0 and top_p >= 1 switch those filters off (the engine's
- * "top_p = 0 means off" is not applied here).  Rows whose slot is done are skipped.
+ * The engine passes its sampler this same struct; every pointer is a device pointer.  Values are
+ * used as given: temperature <= 0 runs the greedy kernel (arg-max, lowest index wins ties),
+ * top_k <= 0 and top_p >= 1 switch those filters off (the engine's "top_p = 0 means off" is not
+ * applied here).  Rows whose slot is done are skipped.
  * out_tau (optional, [B]): for every row the stochastic kernel samples, the order-preserving
  * key of the smallest kept z = logit * (1/T): bits of z with the sign bit set when z >= 0, all
  * bits inverted when z < 0, -0.0 taken as +0.0; 0 when no filter is active.  The kept set is
@@ -135,7 +135,7 @@ typedef struct {
   const int32_t* row_slot;  /* [B] slot of each logits row                                  */
   int32_t* slot_state;      /* per slot: DFA state, -1 = unconstrained (NULL = all -1)      */
   int32_t* slot_ngen;       /* tokens generated so far (Philox step counter)                */
-  int32_t* slot_next_tok;   /* out: the sampled token                                       */
+  int32_t* slot_next_tok;   /* out: the sampled token (the input of the next step)          */
   int32_t* slot_pos;        /* incremented by one                                           */
   int32_t* slot_done;       /* set to 1 when the row ends at this step                      */
   const int32_t* slot_row;  /* output row of each slot                                      */
@@ -145,9 +145,9 @@ typedef struct {
   int out_stride;
   const uint32_t* mask_bits; /* [n_states, mask_words] from sb200_fsm_build_mask, or NULL   */
   int mask_words;
-  const int32_t* fsm_trans;  /* [n_states, 256], -1 = dead                                  */
-  const uint8_t* fsm_accept;
-  const uint8_t* fsm_final;
+  const int32_t* fsm_trans;  /* [n_states, 256] byte transitions, -1 = dead                 */
+  const uint8_t* fsm_accept; /* [n_states]                                                  */
+  const uint8_t* fsm_final;  /* [n_states]: accepting with no outgoing edge                 */
   const int32_t* fsm_tail_off; /* [n_states+1] jump-forward tails, or NULL                  */
   const int32_t* fsm_tail_tok;
   const uint8_t* tok_bytes;  /* vocabulary byte strings                                     */
@@ -157,12 +157,13 @@ typedef struct {
   int top_k;
   float top_p;
   uint64_t seed;
-  int seed_per_row;
-  const int64_t* row_ids;    /* optional [n_rows]: Philox stream id per row                 */
-  float* slot_cum_logprob;   /* optional: running sum of log p(token)                       */
-  float* out_cum_logprob;    /* optional [n_rows]                                           */
+  int seed_per_row;          /* 1: every row draws from its own Philox stream               */
+  const int64_t* row_ids;    /* optional [n_rows]: Philox stream id per row (NULL = row index) */
+  float* slot_cum_logprob;   /* optional: running sum of log p(token) under the masked softmax */
+  float* out_cum_logprob;    /* optional [n_rows], written together with out_len            */
   uint32_t* out_tau;         /* optional [B], see above                                     */
-  /* as in sb200_job (0 = off; repetition_penalty <= 0 is off too); min_p raises out_tau     */
+  /* as in sb200_job (0 = off; repetition_penalty <= 0 is off too); min_p (stochastic kernel
+   * only) raises out_tau                                                                    */
   float presence_penalty, frequency_penalty, repetition_penalty, min_p;
   /* the prompt the penalties count, needed when one is active: prompt_prefix |
    * row_tokens[row_tok_off[row] ..][0, slot_n_row_tok[slot]) | prompt_suffix, row =

@@ -139,54 +139,7 @@ int sb200_fsm_build_mask(const int32_t* fsm_trans, const uint8_t* fsm_accept, in
 }
 
 int sb200_sample(const sb200_sample_args* p, void* stream) {
-  SampleArgs a{};
-  a.logits = p->logits;
-  a.ldl = p->ldl;
-  a.vocab = p->vocab;
-  a.B = p->B;
-  a.row_slot = p->row_slot;
-  a.slot_state = p->slot_state;
-  a.slot_ngen = p->slot_ngen;
-  a.slot_next_tok = p->slot_next_tok;
-  a.slot_pos = p->slot_pos;
-  a.slot_done = p->slot_done;
-  a.slot_row = p->slot_row;
-  a.slot_maxnew = p->slot_maxnew;
-  a.out_tokens = p->out_tokens;
-  a.out_len = p->out_len;
-  a.out_stride = p->out_stride;
-  a.mask_bits = p->mask_bits;
-  a.mask_words = p->mask_words;
-  a.fsm_trans = p->fsm_trans;
-  a.fsm_accept = p->fsm_accept;
-  a.fsm_final = p->fsm_final;
-  a.fsm_tail_off = p->fsm_tail_off;
-  a.fsm_tail_tok = p->fsm_tail_tok;
-  a.tok_bytes = p->tok_bytes;
-  a.tok_off = p->tok_off;
-  a.eos_id = p->eos_id;
-  a.ignore_eos = p->ignore_eos;
-  a.temperature = p->temperature;
-  a.top_k = p->top_k;
-  a.top_p = p->top_p;
-  a.seed = p->seed;
-  a.seed_per_row = p->seed_per_row;
-  a.row_ids = p->row_ids;
-  a.slot_cum_logprob = p->slot_cum_logprob;
-  a.out_cum_logprob = p->out_cum_logprob;
-  a.out_tau = p->out_tau;
-  a.presence_penalty = p->presence_penalty;
-  a.frequency_penalty = p->frequency_penalty;
-  a.repetition_penalty = p->repetition_penalty;
-  a.min_p = p->min_p;
-  a.prompt_prefix = p->prompt_prefix;
-  a.n_prompt_prefix = p->n_prompt_prefix;
-  a.prompt_suffix = p->prompt_suffix;
-  a.n_prompt_suffix = p->n_prompt_suffix;
-  a.row_tokens = p->row_tokens;
-  a.row_tok_off = p->row_tok_off;
-  a.slot_n_row_tok = p->slot_n_row_tok;
-  return sample_greedy(a, STREAM(stream));
+  return sample_greedy(*p, STREAM(stream));
 }
 
 int sb200_tokenizer_create(const int32_t* merges, int n_merges, const int32_t* merged_ids,

@@ -114,6 +114,28 @@ int exclusive_scan_i64(const int64_t* in, int64_t* out, int64_t n, cudaStream_t 
   return 0;
 }
 
+// len[n_rows] (int32) -> off[n_rows+1], the exclusive scan of the lengths widened to int64
+int row_offsets(const int32_t* len, int64_t n_rows, int64_t* off, cudaStream_t stream) {
+  const int64_t n1 = n_rows + 1;
+  int64_t* len64 = nullptr;
+  SB_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&len64), n1 * 8, stream));
+  widen_lengths_kernel<<<static_cast<unsigned>((n1 + 255) / 256), 256, 0, stream>>>(len, len64,
+                                                                                   n_rows);
+  const int rc = exclusive_scan_i64(len64, off, n1, stream);
+  cudaFreeAsync(len64, stream);
+  return rc;
+}
+
+// out_tokens[n_rows, stride] -> flat[off[i] .. off[i+1]), off from row_offsets()
+int compact_rows(const int32_t* out_tokens, int stride, const int64_t* off, int32_t* flat,
+                 int64_t n_rows, cudaStream_t stream) {
+  if (n_rows > 0)
+    compact_rows_kernel<<<static_cast<unsigned>(n_rows), 64, 0, stream>>>(out_tokens, stride, off,
+                                                                           flat, n_rows);
+  SB_CUDA_CHECK(cudaGetLastError());
+  return 0;
+}
+
 template <class T>
 T* host_alloc(size_t n) {
   return static_cast<T*>(std::malloc((n ? n : 1) * sizeof(T)));
@@ -146,19 +168,8 @@ int sb200_compact_rows(const int32_t* out_tokens_dev, const int32_t* out_len_dev
     set_last_error("compact_rows: null argument");
     return -1;
   }
-  const int64_t n1 = n_rows + 1;
-  int64_t* len64 = nullptr;
-  SB_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&len64), n1 * 8, stream));
-  widen_lengths_kernel<<<static_cast<unsigned>((n1 + 255) / 256), 256, 0, stream>>>(
-      out_len_dev, len64, n_rows);
-  const int rc = exclusive_scan_i64(len64, off_dev, n1, stream);
-  cudaFreeAsync(len64, stream);
-  if (rc) return -1;
-  if (n_rows > 0)
-    compact_rows_kernel<<<static_cast<unsigned>(n_rows), 64, 0, stream>>>(
-        out_tokens_dev, stride, off_dev, flat_dev, n_rows);
-  SB_CUDA_CHECK(cudaGetLastError());
-  return 0;
+  if (row_offsets(out_len_dev, n_rows, off_dev, stream)) return -1;
+  return compact_rows(out_tokens_dev, stride, off_dev, flat_dev, n_rows, stream);
 }
 
 // Select m rows (idx, any order, no repeats needed) of a device-resident string column:
@@ -307,12 +318,11 @@ int sb200_infer_text(void* engine, void* tokenizer, const uint8_t* rows_bytes,
     return 0;
   }
 
-  DevBuf d_len64, d_ooff, d_flat, d_boff, d_bytes;
+  DevBuf d_ooff, d_flat, d_boff, d_bytes;
   const int64_t n1 = n_rows + 1;
-  if (d_len64.alloc(n1 * 8) || d_ooff.alloc(n1 * 8)) return -1;
-  widen_lengths_kernel<<<static_cast<unsigned>((n1 + 255) / 256), 256, 0, stream>>>(
-      d_len.as<int32_t>(), d_len64.as<int64_t>(), n_rows);
-  if (exclusive_scan_i64(d_len64.as<int64_t>(), d_ooff.as<int64_t>(), n1, stream)) return -1;
+  if (d_ooff.alloc(n1 * 8) ||
+      row_offsets(d_len.as<int32_t>(), n_rows, d_ooff.as<int64_t>(), stream))
+    return -1;
   r->token_offsets = host_alloc<int64_t>(n1);
   if (!r->token_offsets) {
     set_last_error("infer_text: out of host memory");
@@ -322,11 +332,9 @@ int sb200_infer_text(void* engine, void* tokenizer, const uint8_t* rows_bytes,
                                 stream));
   SB_CUDA_CHECK(cudaStreamSynchronize(stream));
   const int64_t n_out = r->token_offsets[n_rows];
-  if (d_flat.alloc(n_out * 4)) return -1;
-  if (n_rows > 0)
-    compact_rows_kernel<<<static_cast<unsigned>(n_rows), 64, 0, stream>>>(
-        d_out.as<int32_t>(), max_new, d_ooff.as<int64_t>(), d_flat.as<int32_t>(), n_rows);
-  SB_CUDA_CHECK(cudaGetLastError());
+  if (d_flat.alloc(n_out * 4) || compact_rows(d_out.as<int32_t>(), max_new, d_ooff.as<int64_t>(),
+                                              d_flat.as<int32_t>(), n_rows, stream))
+    return -1;
   r->tokens = host_alloc<int32_t>(n_out);
   if (!r->tokens) {
     set_last_error("infer_text: out of host memory");

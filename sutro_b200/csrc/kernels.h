@@ -7,6 +7,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/sutro_b200.h"
+
 namespace sb {
 
 const char* last_error();
@@ -125,60 +127,9 @@ int attn_prefill_q_tile(int hq, int hkv);  // query tokens per work item: 128 / 
 int encode_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims,
                      const uint64_t* strides_bytes, const uint32_t* box);
 
-// K8 — FSM token-mask build, masked greedy sampling + FSM advance.
-struct SampleArgs {
-  float* logits;            // [B, ldl]; rewritten in place when a penalty is active
-  int ldl;
-  int vocab;
-  int B;
-  const int32_t* row_slot;  // [B] slot of each logits row
-  // per-slot decode state
-  int32_t* slot_state;      // FSM state (or -1 when unconstrained)
-  int32_t* slot_ngen;       // tokens generated so far
-  int32_t* slot_next_tok;   // out: sampled token (input of next step)
-  int32_t* slot_pos;        // position of next token (incremented)
-  int32_t* slot_done;       // out: 1 when the row finished at this step
-  const int32_t* slot_row;  // global row id of the slot
-  const int32_t* slot_maxnew;
-  int32_t* out_tokens;      // [n_rows, out_stride]
-  int32_t* out_len;         // [n_rows]
-  int out_stride;
-  // FSM tables (null when no schema)
-  const uint32_t* mask_bits;   // [n_states, mask_words]
-  int mask_words;
-  const int32_t* fsm_trans;    // [n_states, 256] byte transitions, -1 = dead
-  const uint8_t* fsm_accept;   // [n_states]
-  const uint8_t* fsm_final;    // [n_states] accepting with no outgoing edge
-  const int32_t* fsm_tail_off; // [n_states+1] or null: forced terminal continuation per state
-  const int32_t* fsm_tail_tok;
-  const uint8_t* tok_bytes;    // vocab byte blob
-  const int32_t* tok_off;      // [vocab+1]
-  int eos_id;
-  int ignore_eos;
-  // sampling_params (reference: opaque dict forwarded to the service, sutro/sdk.py:203)
-  float temperature;       // 0 = greedy (arg-max, lowest index wins ties)
-  int top_k;               // <= 0: off
-  float top_p;             // >= 1: off
-  uint64_t seed;
-  int seed_per_row;        // random_seed_per_input (sutro/sdk.py:204): 1 = own stream per row
-  const int64_t* row_ids;  // optional [n_rows]: stream id per row (null = row index)
-  float* slot_cum_logprob; // nullable: running sum of log p(token) under the masked softmax
-  float* out_cum_logprob;  // [n_rows], written together with out_len
-  uint32_t* out_tau;       // nullable [B]: order-preserving key of the smallest kept z (stochastic
-                           // kernel only; 0 = no filter).  Kept = allowed and fkey(z) >= tau.
-  // presence / frequency / repetition penalties (vLLM's apply_penalties) over the row's prompt
-  // prefix | row_tokens[row_tok_off[row] ..][0, slot_n_row_tok[slot]) | suffix and its output
-  // out_tokens[row][0, slot_ngen[slot]); min_p (stochastic kernel only).  0 = off, except
-  // repetition_penalty, where <= 0 and 1 are off.
-  const int32_t* prompt_prefix;
-  int n_prompt_prefix;
-  const int32_t* prompt_suffix;
-  int n_prompt_suffix;
-  const int32_t* row_tokens;
-  const int64_t* row_tok_off;
-  const int32_t* slot_n_row_tok;
-  float presence_penalty, frequency_penalty, repetition_penalty, min_p;
-};
+// K8 — FSM token-mask build, masked greedy sampling + FSM advance.  The sampler's arguments are
+// the public sb200_sample_args, documented in the header.
+using SampleArgs = sb200_sample_args;
 // The row-history table of the penalty kernel is sized by out_stride; longer outputs are refused.
 constexpr int kPenaltyMaxOutput = 8192;
 bool penalties_active(const SampleArgs& a);  // sample_greedy() then launches the penalty kernel

@@ -24,6 +24,7 @@
 
 #include "../../include/sutro_b200.h"
 #include "common.cuh"
+#include "dev_buf.h"
 #include "json_mini.h"
 #include "kernels.h"
 
@@ -95,49 +96,33 @@ int encode_texts(Model* m, const std::vector<std::string>& texts,
   }
   const int64_t nb = static_cast<int64_t>(blob.size());
   cudaStream_t stream = static_cast<cudaStream_t>(sb200_engine_stream(m->engine));
-  uint8_t* d_text = nullptr;
-  int64_t *d_off = nullptr, *d_toff = nullptr;
-  int32_t* d_tok = nullptr;
-  auto cleanup = [&] {
-    cudaFree(d_text);
-    cudaFree(d_off);
-    cudaFree(d_toff);
-    cudaFree(d_tok);
-  };
   const size_t n1 = texts.size() + 1;
-  if (cudaMalloc(&d_text, nb ? nb : 1) != cudaSuccess || cudaMalloc(&d_off, n1 * 8) != cudaSuccess ||
-      cudaMalloc(&d_toff, n1 * 8) != cudaSuccess ||
-      cudaMalloc(&d_tok, (nb ? nb : 1) * 4) != cudaSuccess) {
-    cleanup();
+  DevBuf d_text, d_off, d_toff, d_tok;
+  if (d_text.alloc(nb) || d_off.alloc(n1 * 8) || d_toff.alloc(n1 * 8) || d_tok.alloc(nb * 4)) {
     set_last_error("model: out of device memory while tokenising template text");
     return -1;
   }
+  auto cuda_error = [] {
+    set_last_error("model: CUDA error while tokenising template text");
+    return -1;
+  };
+  const cudaMemcpyKind h2d = cudaMemcpyHostToDevice, d2h = cudaMemcpyDeviceToHost;
+  if ((nb && cudaMemcpyAsync(d_text.p, blob.data(), nb, h2d, stream) != cudaSuccess) ||
+      cudaMemcpyAsync(d_off.p, off.data(), n1 * 8, h2d, stream) != cudaSuccess)
+    return cuda_error();
+  if (sb200_tokenizer_encode(m->tokenizer, d_text.as<uint8_t>(), nb, d_off.as<int64_t>(),
+                             static_cast<int64_t>(texts.size()), d_tok.as<int32_t>(),
+                             d_toff.as<int64_t>(), stream))
+    return -1;
   std::vector<int64_t> toff(n1);
-  std::vector<int32_t> toks;
-  int rc = 0;
-  do {
-    if (nb && cudaMemcpyAsync(d_text, blob.data(), nb, cudaMemcpyHostToDevice, stream) != cudaSuccess) rc = -1;
-    if (cudaMemcpyAsync(d_off, off.data(), n1 * 8, cudaMemcpyHostToDevice, stream) != cudaSuccess) rc = -1;
-    if (rc) break;
-    if (sb200_tokenizer_encode(m->tokenizer, d_text, nb, d_off, static_cast<int64_t>(texts.size()),
-                               d_tok, d_toff, stream)) {
-      rc = -2;
-      break;
-    }
-    if (cudaMemcpyAsync(toff.data(), d_toff, n1 * 8, cudaMemcpyDeviceToHost, stream) != cudaSuccess ||
-        cudaStreamSynchronize(stream) != cudaSuccess) {
-      rc = -1;
-      break;
-    }
-    toks.resize(toff.back() > 0 ? toff.back() : 0);
-    if (!toks.empty() &&
-        (cudaMemcpyAsync(toks.data(), d_tok, toks.size() * 4, cudaMemcpyDeviceToHost, stream) != cudaSuccess ||
-         cudaStreamSynchronize(stream) != cudaSuccess))
-      rc = -1;
-  } while (false);
-  cleanup();
-  if (rc == -1) set_last_error("model: CUDA error while tokenising template text");
-  if (rc) return -1;
+  if (cudaMemcpyAsync(toff.data(), d_toff.p, n1 * 8, d2h, stream) != cudaSuccess ||
+      cudaStreamSynchronize(stream) != cudaSuccess)
+    return cuda_error();
+  std::vector<int32_t> toks(toff.back() > 0 ? toff.back() : 0);
+  if (!toks.empty() &&
+      (cudaMemcpyAsync(toks.data(), d_tok.p, toks.size() * 4, d2h, stream) != cudaSuccess ||
+       cudaStreamSynchronize(stream) != cudaSuccess))
+    return cuda_error();
   for (size_t i = 0; i < texts.size(); ++i)
     (*out)[i].assign(toks.begin() + toff[i], toks.begin() + toff[i + 1]);
   return 0;

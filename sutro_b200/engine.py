@@ -82,6 +82,14 @@ class JobStatsC(C.Structure):
                 ("gemm_flops", C.c_double), ("attn_decode_bytes", C.c_double),
                 ("t_h2d_ms", C.c_double), ("t_device_ms", C.c_double), ("t_d2h_ms", C.c_double)]
 
+    def counters(self) -> Dict[str, Any]:
+        """The job's counters as every entry point's stats dict reports them."""
+        stats: Dict[str, Any] = {k: int(getattr(self, k)) for k in _STAT_INTS}
+        stats["kernel_launches"] = dict(zip(KERNEL_CLASSES, list(self.kernel_launches)))
+        stats["kernel_ms"] = dict(zip(KERNEL_CLASSES, list(self.kernel_ms)))
+        stats["gemm_flops"], stats["attn_decode_bytes"] = self.gemm_flops, self.attn_decode_bytes
+        return stats
+
 
 L.register("sb200_engine_create", C.c_int, [C.POINTER(EngineConfigC), C.POINTER(EngineWeightsC),
                                             C.POINTER(C.c_void_p)])
@@ -369,6 +377,31 @@ class GenerationResult:
     cum_logprobs: Optional[np.ndarray] = None  # fp32 [n_rows] when return_logprobs=True
 
 
+@dataclass(frozen=True)
+class JobOptions:
+    """What a job asks for: prompt framing, output schema, output budget and sampling.
+    `generate`, `run_blob_dev` and `infer_one_call` take these fields as keywords; the defaults
+    here are theirs."""
+    system_prompt: Optional[str] = None
+    json_schema: Optional[Dict[str, Any]] = None
+    max_new_tokens: int = 64
+    ignore_eos: bool = False
+    truncate_rows: bool = True
+    share_prefix: bool = True
+    fsm_limits: Optional[FsmLimits] = None
+    jump_forward: bool = True
+    temperature: float = 0.0
+    top_k: int = 0
+    top_p: float = 1.0
+    seed: int = 0
+    seed_per_row: bool = False
+    thinking_chars: Optional[int] = None
+    presence_penalty: float = 0.0
+    frequency_penalty: float = 0.0
+    repetition_penalty: float = 1.0
+    min_p: float = 0.0
+
+
 def default_max_prefill_tokens(spec: MS.ModelSpec) -> int:
     """A prompt is never split over prefill steps, so the default step holds one row that fills
     the context window, and at least 8,192 tokens."""
@@ -512,34 +545,31 @@ class LocalEngine:
                                     else compile_thinking(schema, limits, thinking_chars))
         return self._fsm_cache[key]
 
-    def _job_options(self, job: "JobC", system_prompt, json_schema, max_new_tokens, ignore_eos,
-                     truncate_rows, share_prefix, fsm_limits, jump_forward, temperature, top_k,
-                     top_p, seed, seed_per_row, thinking_chars=None, presence_penalty=0.0,
-                     frequency_penalty=0.0, repetition_penalty=1.0, min_p=0.0):
+    def _job_options(self, job: "JobC", opts: JobOptions):
         """Fill the host-side fields of an sb200_job (prompt framing, schema automaton, jump-forward
         plan, sampling).  Returns (dfa, plan, keep) — `keep` holds the arrays the job points at."""
         emb_mode = self.spec.embedding_model
-        thinking = thinking_chars is not None and not emb_mode
-        pre, suf = self._template_tokens(system_prompt, thinking)
+        thinking = opts.thinking_chars is not None and not emb_mode
+        pre, suf = self._template_tokens(opts.system_prompt, thinking)
         dfa = None
         if thinking:
-            dfa = self.compile_schema(json_schema, fsm_limits, int(thinking_chars))
-        elif json_schema is not None:
-            dfa = self.compile_schema(json_schema, fsm_limits)
+            dfa = self.compile_schema(opts.json_schema, opts.fsm_limits, int(opts.thinking_chars))
+        elif opts.json_schema is not None:
+            dfa = self.compile_schema(opts.json_schema, opts.fsm_limits)
         plan = None
-        if dfa is not None and jump_forward and not emb_mode:
+        if dfa is not None and opts.jump_forward and not emb_mode:
             # jump-forward decoding: bytes the automaton forces are not the model's choice —
             # the forced output prefix rides with the prompt, forced terminal tails are
             # appended by the sampler without another forward pass
             plan = self._jump_plan(dfa, (id(dfa),))
-            if plan is not None and len(plan["prefix_tokens"]) >= max_new_tokens:
+            if plan is not None and len(plan["prefix_tokens"]) >= opts.max_new_tokens:
                 plan = None
         if plan is not None:
             suf = np.concatenate([suf, plan["prefix_tokens"]]).astype(np.int32)
         job.prefix_tokens, job.n_prefix = _np_ptr(pre, c_i32p), len(pre)
         job.suffix_tokens, job.n_suffix = _np_ptr(suf, c_i32p), len(suf)
-        job.share_prefix, job.max_new_tokens = int(share_prefix), max_new_tokens
-        job.ignore_eos, job.truncate_rows = int(ignore_eos), int(truncate_rows)
+        job.share_prefix, job.max_new_tokens = int(opts.share_prefix), opts.max_new_tokens
+        job.ignore_eos, job.truncate_rows = int(opts.ignore_eos), int(opts.truncate_rows)
         if dfa is not None:
             job.fsm_trans = _np_ptr(dfa.trans, c_i32p)
             job.fsm_accept = _np_ptr(dfa.accept, c_u8p)
@@ -550,31 +580,32 @@ class LocalEngine:
                 job.n_forced_prefix = len(plan["prefix_tokens"])
                 job.fsm_tail_off = _np_ptr(plan["tail_off"], c_i32p)
                 job.fsm_tail_tok = _np_ptr(plan["tail_tok"], c_i32p)
-        job.temperature, job.top_k, job.top_p = float(temperature), int(top_k), float(top_p)
-        job.seed, job.seed_per_row = int(seed) & (2 ** 64 - 1), int(seed_per_row)
+        job.temperature, job.top_k = float(opts.temperature), int(opts.top_k)
+        job.top_p = float(opts.top_p)
+        job.seed, job.seed_per_row = int(opts.seed) & (2 ** 64 - 1), int(opts.seed_per_row)
         job.presence_penalty, job.frequency_penalty, job.repetition_penalty, job.min_p = \
-            check_penalties(presence_penalty, frequency_penalty, repetition_penalty, min_p)
+            check_penalties(opts.presence_penalty, opts.frequency_penalty,
+                            opts.repetition_penalty, opts.min_p)
         return dfa, plan, (pre, suf)
 
     def run_blob_dev(self, d_text: torch.Tensor, d_off: torch.Tensor, n_rows: int, n_bytes: int,
-                     system_prompt: Optional[str] = None,
-                     json_schema: Optional[Dict[str, Any]] = None, max_new_tokens: int = 64,
-                     ignore_eos: bool = False, truncate_rows: bool = True,
-                     share_prefix: bool = True, fsm_limits: Optional[FsmLimits] = None,
-                     progress: Optional[Callable[[int, int, int], None]] = None,
+                     *, progress: Optional[Callable[[int, int, int], None]] = None,
                      return_text: bool = True, profile: bool = False,
-                     return_first_logits: bool = False, jump_forward: bool = True,
-                     temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0, seed: int = 0,
-                     seed_per_row: bool = False, return_logprobs: bool = False,
-                     row_ids: Optional[Sequence[int]] = None,
-                     thinking_chars: Optional[int] = None, presence_penalty: float = 0.0,
-                     frequency_penalty: float = 0.0, repetition_penalty: float = 1.0,
-                     min_p: float = 0.0) -> Dict[str, Any]:
+                     return_first_logits: bool = False, return_logprobs: bool = False,
+                     row_ids: Optional[Sequence[int]] = None, **options) -> Dict[str, Any]:
         """Phase B of the hot path, HBM to HBM: a device-resident Arrow column (uint8 bytes +
         int64 offsets[n_rows+1]) -> tokenise -> prefill/decode (+mask) -> detokenise ->
         device-resident results (`d_bytes`/`d_boff`, `flat`/`ooff` tokens, `d_emb`, ...).
         Used by generate() and by the row-sharded multi-GPU path (sharding.py), which moves
-        these buffers between ranks over NCCL."""
+        these buffers between ranks over NCCL.  `options`: the fields of JobOptions."""
+        return self._run_blob_dev(d_text, d_off, n_rows, n_bytes, JobOptions(**options),
+                                  progress=progress, return_text=return_text, profile=profile,
+                                  return_first_logits=return_first_logits,
+                                  return_logprobs=return_logprobs, row_ids=row_ids)
+
+    def _run_blob_dev(self, d_text, d_off, n_rows, n_bytes, opts: JobOptions, *, progress,
+                      return_text, profile, return_first_logits, return_logprobs, row_ids):
+        max_new_tokens = opts.max_new_tokens
         dev = self.device
         emb_mode = self.spec.embedding_model
         lib = L.lib()
@@ -593,11 +624,7 @@ class LocalEngine:
                 d_len = torch.zeros(n_rows, dtype=torch.int32, device=dev)
             cb = PROGRESS_FN(lambda r, i, o, u: progress(r, i, o)) if progress else PROGRESS_FN()
             job = JobC()
-            dfa, plan, keep = self._job_options(job, system_prompt, json_schema, max_new_tokens,
-                                                ignore_eos, truncate_rows, share_prefix, fsm_limits,
-                                                jump_forward, temperature, top_k, top_p, seed,
-                                                seed_per_row, thinking_chars, presence_penalty,
-                                                frequency_penalty, repetition_penalty, min_p)
+            dfa, plan, keep = self._job_options(job, opts)
             job.row_tokens_dev, job.row_tok_off_dev = d_tok.data_ptr(), d_toff.data_ptr()
             job.row_tok_off, job.n_rows = _np_ptr(toff, c_i64p), n_rows
             job.out_tokens_dev = L.ptr(d_out)
@@ -610,7 +637,7 @@ class LocalEngine:
                 d_first = torch.zeros(n_rows, self.spec.vocab_size, dtype=torch.float32, device=dev)
                 job.out_first_logits_dev = d_first.data_ptr()
             d_ids = None
-            if row_ids is not None and seed_per_row:
+            if row_ids is not None and opts.seed_per_row:
                 # rows of a sharded job keep the Philox stream of their index in the whole job
                 ids = np.ascontiguousarray(row_ids, dtype=np.int64)
                 if ids.shape != (n_rows,):
@@ -650,10 +677,7 @@ class LocalEngine:
                                                        L.current_stream()))
                     d_bytes = d_bytes[:total]
             torch.cuda.synchronize(dev)
-        stats = {k: int(getattr(st, k)) for k in _STAT_INTS}
-        stats["kernel_launches"] = dict(zip(KERNEL_CLASSES, list(st.kernel_launches)))
-        stats["kernel_ms"] = dict(zip(KERNEL_CLASSES, list(st.kernel_ms)))
-        stats["gemm_flops"], stats["attn_decode_bytes"] = st.gemm_flops, st.attn_decode_bytes
+        stats = st.counters()
         # my kernels outside the engine: tokenizer encode (4), compaction (widen + scan + compact)
         # and decode (2 passes: 2 + 3)
         stats["tokenizer_launches"] = 4 + (0 if emb_mode else 3) + \
@@ -679,26 +703,17 @@ class LocalEngine:
                                               L.current_stream()))
         return out_off, out_bytes
 
-    def generate(self, rows, system_prompt: Optional[str] = None,
-                 json_schema: Optional[Dict[str, Any]] = None, max_new_tokens: int = 64,
-                 ignore_eos: bool = False, truncate_rows: bool = True, share_prefix: bool = True,
-                 fsm_limits: Optional[FsmLimits] = None,
-                 progress: Optional[Callable[[int, int, int], None]] = None,
-                 return_tokens: bool = False, return_text: bool = True,
-                 profile: bool = False, return_first_logits: bool = False,
-                 jump_forward: bool = True, temperature: float = 0.0, top_k: int = 0,
-                 top_p: float = 1.0, seed: int = 0, seed_per_row: bool = False,
-                 return_logprobs: bool = False,
-                 row_ids: Optional[Sequence[int]] = None,
-                 thinking_chars: Optional[int] = None, presence_penalty: float = 0.0,
-                 frequency_penalty: float = 0.0, repetition_penalty: float = 1.0,
-                 min_p: float = 0.0) -> GenerationResult:
+    def generate(self, rows, *, progress: Optional[Callable[[int, int, int], None]] = None,
+                 return_tokens: bool = False, return_text: bool = True, profile: bool = False,
+                 return_first_logits: bool = False, return_logprobs: bool = False,
+                 row_ids: Optional[Sequence[int]] = None, **options) -> GenerationResult:
         """The whole hot path for one frame column.  Three phases, timed separately:
           A  host -> HBM   : rows -> Arrow blob, template/schema compile (cached), H2D copy
           B  device        : tokenize, prefill/decode (+mask), detokenize — HBM to HBM
           C  HBM -> host   : D2H of bytes/offsets, Python strings
         stats["t_device_s"] is phase B alone (inputs resident in HBM), stats["t_total_s"]
-        is A+B+C."""
+        is A+B+C.  `options`: the fields of JobOptions."""
+        opts = JobOptions(**options)
         dev = self.device
         emb_mode = self.spec.embedding_model
         t0 = time.perf_counter()
@@ -712,9 +727,9 @@ class LocalEngine:
                                     else None, {"n_rows": 0, "input_tokens": 0,
                                                 "output_tokens": 0, "rows_done": 0})
         # template / schema compilation (cached) belongs to the host phase
-        self._template_tokens(system_prompt, thinking_chars is not None)
-        if json_schema is not None or thinking_chars is not None:
-            self.compile_schema(json_schema, fsm_limits, thinking_chars)
+        self._template_tokens(opts.system_prompt, opts.thinking_chars is not None)
+        if opts.json_schema is not None or opts.thinking_chars is not None:
+            self.compile_schema(opts.json_schema, opts.fsm_limits, opts.thinking_chars)
         with torch.cuda.device(dev):
             d_text = (torch.from_numpy(np.ascontiguousarray(data)).to(dev) if n_bytes
                       else torch.zeros(1, dtype=torch.uint8, device=dev))
@@ -722,19 +737,10 @@ class LocalEngine:
             torch.cuda.synchronize(dev)
             t_a = time.perf_counter()
             # ---- phase B ---------------------------------------------------------
-            r = self.run_blob_dev(d_text, d_off, n_rows, n_bytes, system_prompt=system_prompt,
-                                  json_schema=json_schema, max_new_tokens=max_new_tokens,
-                                  ignore_eos=ignore_eos, truncate_rows=truncate_rows,
-                                  share_prefix=share_prefix, fsm_limits=fsm_limits,
-                                  progress=progress, return_text=return_text, profile=profile,
-                                  return_first_logits=return_first_logits,
-                                  jump_forward=jump_forward, temperature=temperature, top_k=top_k,
-                                  top_p=top_p, seed=seed, seed_per_row=seed_per_row,
-                                  return_logprobs=return_logprobs, row_ids=row_ids,
-                                  thinking_chars=thinking_chars,
-                                  presence_penalty=presence_penalty,
-                                  frequency_penalty=frequency_penalty,
-                                  repetition_penalty=repetition_penalty, min_p=min_p)
+            r = self._run_blob_dev(d_text, d_off, n_rows, n_bytes, opts, progress=progress,
+                                   return_text=return_text, profile=profile,
+                                   return_first_logits=return_first_logits,
+                                   return_logprobs=return_logprobs, row_ids=row_ids)
             t_b = time.perf_counter()
             # ---- phase C ---------------------------------------------------------
             outputs = out_tokens = emb = None
@@ -761,85 +767,66 @@ class LocalEngine:
                                 None if r["d_first"] is None else r["d_first"].cpu(),
                                 None if r["d_lp"] is None else r["d_lp"].cpu().numpy())
 
-
-def _infer_one_call(self, rows, system_prompt: Optional[str] = None,
-                    json_schema: Optional[Dict[str, Any]] = None, max_new_tokens: int = 64,
-                    ignore_eos: bool = False, truncate_rows: bool = True,
-                    share_prefix: bool = True, fsm_limits: Optional[FsmLimits] = None,
-                    jump_forward: bool = True, temperature: float = 0.0, top_k: int = 0,
-                    top_p: float = 1.0, seed: int = 0, seed_per_row: bool = False,
-                    return_logprobs: bool = False, return_tokens: bool = True,
-                    progress: Optional[Callable[[int, int, int], None]] = None,
-                    profile: bool = False,
-                    thinking_chars: Optional[int] = None, presence_penalty: float = 0.0,
-                    frequency_penalty: float = 0.0, repetition_penalty: float = 1.0,
-                    min_p: float = 0.0) -> GenerationResult:
-    """The same job through `sb200_infer_text`: ONE C-ABI call with host buffers in and out
-    (what a non-Python host would bind; the SDK's infer() and bench.py's `e2e` use it).
-    `generate` is the phased form of the same work; the results are identical.  The call times
-    its three phases with CUDA events on the engine's stream: stats["t_h2d_ms"] (rows -> HBM),
-    stats["t_device_ms"] (tokenise -> prefill/decode -> detokenise, HBM to HBM) and
-    stats["t_d2h_ms"]."""
-    rows = normalize_rows(rows, self.vocab)
-    t0 = time.perf_counter()
-    data, off = rows_to_blob(rows)
-    n_rows = len(off) - 1
-    emb_mode = self.spec.embedding_model
-    data, off = np.ascontiguousarray(data), np.ascontiguousarray(off, dtype=np.int64)
-    job = JobC()
-    dfa, plan, keep = self._job_options(job, system_prompt, json_schema, max_new_tokens,
-                                        ignore_eos, truncate_rows, share_prefix, fsm_limits,
-                                        jump_forward, temperature, top_k, top_p, seed, seed_per_row,
-                                        thinking_chars, presence_penalty, frequency_penalty,
-                                        repetition_penalty, min_p)
-    cb = PROGRESS_FN(lambda r, i, o, u: progress(r, i, o)) if progress else PROGRESS_FN()
-    job.progress = cb
-    job.profile = int(profile)
-    st, res = JobStatsC(), C.POINTER(ResultC)()
-    t1 = time.perf_counter()
-    L.check(L.lib().sb200_infer_text(self._h, self.tokenizer._h, data.ctypes.data, off.ctypes.data,
-                                     n_rows, C.byref(job), 1, int(return_logprobs),
-                                     C.byref(res), C.byref(st)))
-    t2 = time.perf_counter()
-    n_out = d2h = 0
-    try:
-        r = res.contents
-        outputs = out_tokens = emb = lp = None
-        if emb_mode:
-            emb = np.ctypeslib.as_array(r.embeddings, shape=(n_rows, r.d_model)).copy() \
-                if n_rows else np.zeros((0, self.spec.d_model), np.float32)
-            d2h = emb.nbytes
-        else:
-            toff = np.ctypeslib.as_array(r.token_offsets, shape=(n_rows + 1,)).copy()
-            n_out = int(toff[-1])
-            if return_tokens:
-                toks = (np.ctypeslib.as_array(r.tokens, shape=(n_out,)).copy()
-                        if n_out else np.zeros(0, np.int32))
-                out_tokens = [toks[toff[i]:toff[i + 1]].tolist() for i in range(n_rows)]
-            boff = np.ctypeslib.as_array(r.offsets, shape=(n_rows + 1,)).copy()
-            blob = (np.ctypeslib.as_array(r.bytes, shape=(int(boff[-1]),)).copy()
-                    if boff[-1] else np.zeros(0, np.uint8))
-            outputs = blob_to_rows(blob, boff)
-            d2h = int(blob.nbytes + boff.nbytes + toff.nbytes + 4 * n_out)
-            if return_logprobs and n_rows:
-                lp = np.ctypeslib.as_array(r.cum_logprob, shape=(n_rows,)).copy()
-    finally:
-        L.lib().sb200_result_free(res)
-    stats = {k: int(getattr(st, k)) for k in _STAT_INTS}
-    stats["kernel_launches"] = dict(zip(KERNEL_CLASSES, list(st.kernel_launches)))
-    stats["kernel_ms"] = dict(zip(KERNEL_CLASSES, list(st.kernel_ms)))
-    stats["gemm_flops"], stats["attn_decode_bytes"] = st.gemm_flops, st.attn_decode_bytes
-    stats["tokenizer_launches"] = 4 + (0 if emb_mode else 3 + 5)
-    stats.update(n_rows=n_rows, output_tokens=n_out, t_total_s=time.perf_counter() - t0,
-                 t_call_s=t2 - t1, t_h2d_ms=st.t_h2d_ms, t_device_ms=st.t_device_ms,
-                 t_d2h_ms=st.t_d2h_ms, t_device_s=st.t_device_ms * 1e-3,
-                 h2d_bytes=int(data.nbytes + off.nbytes), d2h_bytes=int(d2h),
-                 fsm_states=0 if dfa is None else dfa.n_states, jump_forward=plan is not None,
-                 forced_prefix_tokens=0 if plan is None else int(len(plan["prefix_tokens"])))
-    return GenerationResult(outputs, out_tokens, emb, stats, None, lp)
-
-
-LocalEngine.infer_one_call = _infer_one_call
+    def infer_one_call(self, rows, *, return_logprobs: bool = False, return_tokens: bool = True,
+                       progress: Optional[Callable[[int, int, int], None]] = None,
+                       profile: bool = False, **options) -> GenerationResult:
+        """The same job through `sb200_infer_text`: ONE C-ABI call with host buffers in and out
+        (what a non-Python host would bind; the SDK's infer() and bench.py's `e2e` use it).
+        `generate` is the phased form of the same work; the results are identical.  The call times
+        its three phases with CUDA events on the engine's stream: stats["t_h2d_ms"] (rows -> HBM),
+        stats["t_device_ms"] (tokenise -> prefill/decode -> detokenise, HBM to HBM) and
+        stats["t_d2h_ms"].  `options`: the fields of JobOptions."""
+        opts = JobOptions(**options)
+        rows = normalize_rows(rows, self.vocab)
+        t0 = time.perf_counter()
+        data, off = rows_to_blob(rows)
+        n_rows = len(off) - 1
+        emb_mode = self.spec.embedding_model
+        data, off = np.ascontiguousarray(data), np.ascontiguousarray(off, dtype=np.int64)
+        job = JobC()
+        dfa, plan, keep = self._job_options(job, opts)
+        cb = PROGRESS_FN(lambda r, i, o, u: progress(r, i, o)) if progress else PROGRESS_FN()
+        job.progress = cb
+        job.profile = int(profile)
+        st, res = JobStatsC(), C.POINTER(ResultC)()
+        t1 = time.perf_counter()
+        L.check(L.lib().sb200_infer_text(self._h, self.tokenizer._h, data.ctypes.data,
+                                         off.ctypes.data, n_rows, C.byref(job), 1,
+                                         int(return_logprobs), C.byref(res), C.byref(st)))
+        t2 = time.perf_counter()
+        n_out = d2h = 0
+        try:
+            r = res.contents
+            outputs = out_tokens = emb = lp = None
+            if emb_mode:
+                emb = np.ctypeslib.as_array(r.embeddings, shape=(n_rows, r.d_model)).copy() \
+                    if n_rows else np.zeros((0, self.spec.d_model), np.float32)
+                d2h = emb.nbytes
+            else:
+                toff = np.ctypeslib.as_array(r.token_offsets, shape=(n_rows + 1,)).copy()
+                n_out = int(toff[-1])
+                if return_tokens:
+                    toks = (np.ctypeslib.as_array(r.tokens, shape=(n_out,)).copy()
+                            if n_out else np.zeros(0, np.int32))
+                    out_tokens = [toks[toff[i]:toff[i + 1]].tolist() for i in range(n_rows)]
+                boff = np.ctypeslib.as_array(r.offsets, shape=(n_rows + 1,)).copy()
+                blob = (np.ctypeslib.as_array(r.bytes, shape=(int(boff[-1]),)).copy()
+                        if boff[-1] else np.zeros(0, np.uint8))
+                outputs = blob_to_rows(blob, boff)
+                d2h = int(blob.nbytes + boff.nbytes + toff.nbytes + 4 * n_out)
+                if return_logprobs and n_rows:
+                    lp = np.ctypeslib.as_array(r.cum_logprob, shape=(n_rows,)).copy()
+        finally:
+            L.lib().sb200_result_free(res)
+        stats = st.counters()
+        stats["tokenizer_launches"] = 4 + (0 if emb_mode else 3 + 5)
+        stats.update(n_rows=n_rows, output_tokens=n_out, t_total_s=time.perf_counter() - t0,
+                     t_call_s=t2 - t1, t_h2d_ms=st.t_h2d_ms, t_device_ms=st.t_device_ms,
+                     t_d2h_ms=st.t_d2h_ms, t_device_s=st.t_device_ms * 1e-3,
+                     h2d_bytes=int(data.nbytes + off.nbytes), d2h_bytes=int(d2h),
+                     fsm_states=0 if dfa is None else dfa.n_states, jump_forward=plan is not None,
+                     forced_prefix_tokens=0 if plan is None else int(len(plan["prefix_tokens"])))
+        return GenerationResult(outputs, out_tokens, emb, stats, None, lp)
 
 
 # --------------------------------------------------------------------------- several GPUs, one process

@@ -58,3 +58,40 @@ def build_cache(k_seqs, v_seqs, hkv, num_pages, device, seed=0):
             pool[page, :, 0] = pack_tile(kt)
             pool[page, :, 1] = pack_tile(vt)
     return pool, pt.to(device), max_pages
+
+
+# ---- long positions -------------------------------------------------------------------------
+MAX_POS = 32768                   # the longest window the engine serves
+MAX_PAGES = MAX_POS // PAGE + 1   # the engine's page-table width: 2,049 entries
+# positions every long-position test includes: each end of the first splits, 16k and the last
+EDGE_POSITIONS = (0, 4095, 4096, 8191, 8192, 16384, 32767)
+
+
+def long_positions(M, n_slots, seed):
+    """M tokens over n_slots slots (token i in slot i % n_slots) at positions distinct per slot,
+    drawn from [0, 32,768); every slot with at least 7 tokens holds all of EDGE_POSITIONS, at
+    shuffled token indices.  -> (tok_slot, tok_pos) int64 on the CPU."""
+    g = torch.Generator().manual_seed(seed)
+    edges = torch.tensor(EDGE_POSITIONS)
+    tok_slot = torch.arange(M) % n_slots
+    tok_pos = torch.empty(M, dtype=torch.long)
+    for s in range(n_slots):
+        idx = (tok_slot == s).nonzero().flatten()
+        rest = torch.randperm(MAX_POS, generator=g)
+        pos = torch.cat([edges, rest[~torch.isin(rest, edges)]])[:len(idx)]
+        tok_pos[idx] = pos[torch.randperm(len(idx), generator=g)]
+    return tok_slot, tok_pos
+
+
+def sparse_page_table(tok_slot, tok_pos, n_slots, seed, spare=16):
+    """The engine's [n_slots, 2,049] page table over a pool holding only the pages the tokens
+    touch (shuffled ids) and `spare` pages nothing maps; every other entry points at one
+    sentinel page, which no write may reach.  -> (page table int32 cpu, num_pages, sentinel)."""
+    g = torch.Generator().manual_seed(seed)
+    used = torch.unique(tok_slot * MAX_PAGES + tok_pos // PAGE)
+    num_pages = len(used) + 1 + spare
+    ids = torch.randperm(num_pages, generator=g).to(torch.int32)
+    sentinel = int(ids[-1])
+    pt = torch.full((n_slots, MAX_PAGES), sentinel, dtype=torch.int32)
+    pt.view(-1)[used] = ids[:len(used)]
+    return pt, num_pages, sentinel

@@ -17,8 +17,9 @@ GQA group sizes and the engine's scale 1/sqrt(128):
 3. Tight numerics at engine-sized contexts (up to 4096 tokens, ~1000 prefix rows, hundreds of
    decode rows) against an fp64 softmax, with the per-element bound of `error_bound`.
 4. The fused QKV epilogue writes post-norm/RoPE K and V both to the paged pool and, unswizzled,
-   to the k/v columns of its output; the two copies must be identical, and the chain the engine
-   runs (fused QKV -> dense prefill attention) must meet the bound of 3.
+   to the k/v columns of its output; the two copies must be identical, Q and K must be the exact
+   norm -> RoPE of the projection at every served head layout and at positions up to 32,767, and
+   the chain the engine runs (fused QKV -> dense prefill attention) must meet the bound of 3.
 """
 import math
 import random
@@ -27,6 +28,7 @@ import pytest
 import torch
 
 from sutro_b200 import _lib as L
+from sutro_b200 import modelspec as MS
 import bf16_ref as R
 import kv_layout as KV
 
@@ -717,35 +719,48 @@ def fused_qkv(a, m, w, qn, kn, cos, sin, tok_slot, tok_pos, pt, pool, hq, hkv, b
     torch.cuda.synchronize()
 
 
+# every head layout the engine serves: tiny-qwen3 / tiny-llama, tiny-qwen3-g4, qwen-3-0.6b and the
+# embedding model, qwen-3-4b and llama-3.1-8b.  At hkv = 2 one 512-wide tile holds K and V.
+SERVED_HEADS = [(4, 2), (8, 2), (16, 8), (32, 8)]
+SERVED_HEAD_IDS = ["4_2", "8_2", "16_8", "32_8"]
+_TABLES = {}
+
+
+def model_rope_tables(name):
+    """The engine's bf16 cos/sin tables of a real model at all 32,768 positions, on the GPU."""
+    if name not in _TABLES:
+        _TABLES[name] = tuple(t.to(DEV) for t in MS.rope_tables(MS.get_spec(name), KV.MAX_POS))
+    return _TABLES[name]
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("M", [77, 129, 300])
 @pytest.mark.parametrize("qk_norm", [True, False], ids=["qk_norm", "no_norm"])
 @pytest.mark.parametrize("block_n", [0, 128, 256, 512])
-def test_qkv_epilogue_dense_kv_copy(block_n, qk_norm, M):
+@pytest.mark.parametrize("hq,hkv", SERVED_HEADS, ids=SERVED_HEAD_IDS)
+def test_qkv_epilogue_dense_kv_copy(hq, hkv, block_n, qk_norm, M):
     """Small-integer A and W make the projection exact.  The k/v columns of the output must be
     bit-identical to what the same launch wrote into the pool, V must be bf16(A Wv^T), Q and K
-    must match linear -> bf16 -> RMSNorm -> RoPE bit for bit, at positions up to 4095; with the
-    norm, an output whose normed operand (dim i or i + 64) is tied may take either rounding of it
-    (bf16_ref: the epilogue rounds x * rstd to bf16 and then uses exact bf16x2 products, so the
-    window of the fp32 sum of squares and rsqrtf is all that matters).  Output rows >= M and pool
-    slots no token maps to stay untouched."""
-    hq, hkv, K, extra = 32, 8, 256, 40
+    must match linear -> bf16 -> RMSNorm -> RoPE bit for bit, at positions up to 32,767 with the
+    tables of qwen-3-4b (with the norm) or llama-3.1-8b (without); with the norm, an output whose
+    normed operand (dim i or i + 64) is tied may take either rounding of it (bf16_ref: the
+    epilogue rounds x * rstd to bf16 and then uses exact bf16x2 products, so the window of the
+    fp32 sum of squares and rsqrtf is all that matters).  Output rows >= M, pool slots no token
+    maps to and the sentinel page every other page-table entry points at stay untouched.  K < 2,048
+    and one tile per CTA: the consumer warpgroups run the epilogue math."""
+    K, extra = 256, 40
     N = (hq + 2 * hkv) * HD
-    torch.manual_seed(M + block_n + int(qk_norm))
+    torch.manual_seed(M + block_n + int(qk_norm) + hq + hkv)
     a = bf(torch.randint(-2, 3, (M + extra, K), device=DEV).float())
     w = bf(torch.randint(-1, 2, (N, K), device=DEV).float())
     qn = bf(torch.rand(HD, device=DEV) + 0.5) if qk_norm else None
     kn = bf(torch.rand(HD, device=DEV) + 0.5) if qk_norm else None
-    cos, sin = rope_tables(4096)
-    n_slots, max_pages = 4, 4096 // PAGE
-    tok_slot = torch.arange(M) % n_slots
-    tok_pos = torch.empty(M, dtype=torch.long)
-    for s in range(n_slots):
-        idx = (tok_slot == s).nonzero().flatten()
-        tok_pos[idx] = torch.randperm(4095)[:len(idx)]
-    tok_pos[0] = 4095
-    num_pages = n_slots * max_pages + 16
-    pt = torch.randperm(num_pages)[:n_slots * max_pages].view(n_slots, max_pages)
+    cos, sin = model_rope_tables("qwen-3-4b" if qk_norm else "llama-3.1-8b")
+    n_slots = 4
+    tok_slot, tok_pos = KV.long_positions(M, n_slots, seed=M + hq)
+    assert set(KV.EDGE_POSITIONS) <= set(tok_pos.tolist())
+    assert (tok_pos >= 4096).float().mean() > 0.5
+    pt, num_pages, sentinel = KV.sparse_page_table(tok_slot, tok_pos, n_slots, seed=M + block_n)
     pool = torch.full((num_pages, hkv, 2, PAGE, HD), -3.0, dtype=torch.bfloat16, device=DEV)
     out = torch.full((M + extra, N), 7.0, dtype=torch.bfloat16, device=DEV)
     fused_qkv(a, M, w, qn, kn, cos, sin, tok_slot, tok_pos, pt, pool, hq, hkv, block_n, out)
@@ -758,6 +773,7 @@ def test_qkv_epilogue_dense_kv_copy(block_n, qk_norm, M):
     written = torch.zeros(num_pages, PAGE, dtype=torch.bool, device=DEV)
     written[page, r] = True
     assert torch.all(logical.permute(0, 3, 1, 2, 4)[~written] == -3.0), "unmapped pool slots written"
+    assert not written[sentinel].any() and torch.all(logical[sentinel] == -3.0), "sentinel written"
     assert torch.equal(got[:, hq:hq + hkv], logical[page, :, 0, r]), "dense K != paged K"
     assert torch.equal(got[:, hq + hkv:], logical[page, :, 1, r]), "dense V != paged V"
     assert torch.equal(got[:, hq + hkv:], lin[:, hq + hkv:]), "V != bf16(A Wv^T)"
@@ -768,7 +784,7 @@ def test_qkv_epilogue_dense_kv_copy(block_n, qk_norm, M):
                                                sin[pos])
         R.assert_one_of(got[:, sl], cands, name)
         if qk_norm:
-            print(f"[ties] fused QKV {name} M={M} block_n={block_n}: "
+            print(f"[ties] fused QKV {hq}/{hkv} {name} M={M} block_n={block_n}: "
                   f"{tied.double().mean().item():.2e} tied")
             assert tied.double().mean().item() < 0.01, name
 

@@ -15,6 +15,7 @@ import torch
 from sutro_b200 import _lib as L
 import bf16_ref as R
 import kv_layout as KV
+import test_attention_exact_gpu as AX
 
 DEV = "cuda"
 HD, PAGE = KV.HD, KV.PAGE
@@ -36,12 +37,13 @@ def rope_tables(max_pos=4096, theta=1e6):
     return bf(fr.cos()).to(DEV), bf(fr.sin()).to(DEV)
 
 
-def fused_qkv(a, m, w, qn, kn, cos, sin, tok_slot, tok_pos, pt, pool, block_n, out):
+def fused_qkv(a, m, w, qn, kn, cos, sin, tok_slot, tok_pos, pt, pool, block_n, out, hq=HQ,
+              hkv=HKV):
     d_slot, d_pos, d_pt = i32(tok_slot), i32(tok_pos), i32(pt)
     L.check(L.lib().sb200_gemm_qkv_rope(
         L.ptr(a), a.shape[0], L.ptr(w), L.ptr(out), m, a.shape[1], block_n, L.ptr(qn), L.ptr(kn),
         L.ptr(cos), L.ptr(sin), L.ptr(d_slot), L.ptr(d_pos), L.ptr(d_pt), pt.shape[1],
-        L.ptr(pool), HQ, HKV, 1e-6, L.current_stream()))
+        L.ptr(pool), hq, hkv, 1e-6, L.current_stream()))
     torch.cuda.synchronize()
 
 
@@ -64,39 +66,49 @@ def token_layout(M, n_slots, seed):
 @pytest.mark.parametrize("qk_norm", [True, False], ids=["qk_norm", "no_norm"])
 @pytest.mark.parametrize("block_n", [128, 256, 512])
 @pytest.mark.parametrize("K", [2048, 2560])
-def test_qkv_epilogue_warps_many_tiles(K, block_n, qk_norm):
-    """129 row tiles (the last one 77 rows) x 48 or 24 column tiles over the SMs, with K = 2048
-    (the shortest K that takes the epilogue warps) or 2560.  Small-integer A and W make the
-    projection exact (fp32 sums of integers; only the rounding to bf16 remains),
-    so V must be bf16(A Wv^T) and Q and K must be one of the candidates of linear -> bf16 ->
-    RMSNorm -> RoPE; the dense K/V copy must equal the paged one; rows >= M and pool slots no
-    token maps to stay untouched."""
+@pytest.mark.parametrize("hq,hkv", AX.SERVED_HEADS, ids=AX.SERVED_HEAD_IDS)
+def test_qkv_epilogue_warps_many_tiles(hq, hkv, K, block_n, qk_norm):
+    """129 row tiles (the last one 77 rows) x up to 48 column tiles over the SMs, with K = 2048
+    (the shortest K that takes the epilogue warps) or 2560, at every served head layout.  Small-
+    integer A and W make the projection exact (fp32 sums of integers; only the rounding to bf16
+    remains), so V must be bf16(A Wv^T) and Q and K must be one of the candidates of linear ->
+    bf16 -> RMSNorm -> RoPE, with the tables of qwen-3-4b (norm) or llama-3.1-8b (no norm) at
+    positions up to 32,767; the dense K/V copy must equal the paged one; rows >= M, pool slots no
+    token maps to and the sentinel page of the unmapped page-table entries stay untouched."""
     M, extra = 129 * 128 - 51, 40
-    torch.manual_seed(K + block_n + int(qk_norm))
+    N = (hq + 2 * hkv) * HD
+    # more tiles than SMs (even at the widest tile) and K >= 2048: the epilogue warps run
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    assert K >= 2048 and math.ceil(M / 128) * math.ceil(N / 512) > sms
+    torch.manual_seed(K + block_n + int(qk_norm) + hq + hkv)
     a = bf(torch.randint(-2, 3, (M + extra, K), device=DEV).float())
-    w = bf(torch.randint(-1, 2, (N_QKV, K), device=DEV).float())
+    w = bf(torch.randint(-1, 2, (N, K), device=DEV).float())
     qn = bf(torch.rand(HD, device=DEV) + 0.5) if qk_norm else None
     kn = bf(torch.rand(HD, device=DEV) + 0.5) if qk_norm else None
-    cos, sin = rope_tables(4096)
-    tok_slot, tok_pos, pt, num_pages = token_layout(M, 8, seed=K + block_n)
-    pool = torch.full((num_pages, HKV, 2, PAGE, HD), -3.0, dtype=torch.bfloat16, device=DEV)
-    out = torch.full((M + extra, N_QKV), 7.0, dtype=torch.bfloat16, device=DEV)
-    fused_qkv(a, M, w, qn, kn, cos, sin, tok_slot, tok_pos, pt, pool, block_n, out)
+    cos, sin = AX.model_rope_tables("qwen-3-4b" if qk_norm else "llama-3.1-8b")
+    tok_slot, tok_pos = KV.long_positions(M, 8, seed=K + block_n)
+    assert set(KV.EDGE_POSITIONS) <= set(tok_pos.tolist())
+    assert (tok_pos >= 4096).float().mean() > 0.5
+    pt, num_pages, sentinel = KV.sparse_page_table(tok_slot, tok_pos, 8, seed=K + hq)
+    pool = torch.full((num_pages, hkv, 2, PAGE, HD), -3.0, dtype=torch.bfloat16, device=DEV)
+    out = torch.full((M + extra, N), 7.0, dtype=torch.bfloat16, device=DEV)
+    fused_qkv(a, M, w, qn, kn, cos, sin, tok_slot, tok_pos, pt, pool, block_n, out, hq, hkv)
 
-    lin = bf(a[:M].float() @ w.float().t()).view(M, HQ + 2 * HKV, HD)   # exact, then rounded
-    got = out[:M].view(M, HQ + 2 * HKV, HD)
+    lin = bf(a[:M].float() @ w.float().t()).view(M, hq + 2 * hkv, HD)   # exact, then rounded
+    got = out[:M].view(M, hq + 2 * hkv, HD)
     assert torch.all(out[M:] == 7.0), "rows >= M written"
     logical = KV.unpack_tile(pool)
     page, r = pt[tok_slot, tok_pos // PAGE].to(DEV), (tok_pos % PAGE).to(DEV)
     written = torch.zeros(num_pages, PAGE, dtype=torch.bool, device=DEV)
     written[page, r] = True
     assert torch.all(logical.permute(0, 3, 1, 2, 4)[~written] == -3.0), "unmapped pool slots written"
-    assert torch.equal(got[:, HQ:HQ + HKV], logical[page, :, 0, r]), "dense K != paged K"
-    assert torch.equal(got[:, HQ + HKV:], logical[page, :, 1, r]), "dense V != paged V"
-    assert torch.equal(got[:, HQ + HKV:], lin[:, HQ + HKV:]), "V != bf16(A Wv^T)"
+    assert not written[sentinel].any() and torch.all(logical[sentinel] == -3.0), "sentinel written"
+    assert torch.equal(got[:, hq:hq + hkv], logical[page, :, 0, r]), "dense K != paged K"
+    assert torch.equal(got[:, hq + hkv:], logical[page, :, 1, r]), "dense V != paged V"
+    assert torch.equal(got[:, hq + hkv:], lin[:, hq + hkv:]), "V != bf16(A Wv^T)"
 
     pos = tok_pos.to(DEV)
-    for name, sl, nw in (("q", slice(0, HQ), qn), ("k", slice(HQ, HQ + HKV), kn)):
+    for name, sl, nw in (("q", slice(0, hq), qn), ("k", slice(hq, hq + hkv), kn)):
         cands, tied = R.normed_rope_candidates(lin[:, sl], nw, 1e-6, R.QKV_NORM_DEPTH, cos[pos],
                                                sin[pos])
         R.assert_one_of(got[:, sl], cands, name)

@@ -12,7 +12,9 @@ engine serving rows longer than the 4,096-token split.
    against fp64 on a sample of query rows that includes the last.
 3. The engine with 16,384-token windows on the tiny models: rows of ~5k, 9k and 15k tokens among
    short ones, bit-identical to the one-row replay (tests/engine_replay.py) greedy, sampled and
-   under a schema with jump-forward; a system prompt longer than 4,096 tokens (every row split);
+   under a schema with jump-forward; rows that cross a split boundary during decode (4,096 ->
+   4,097 and 8,192 -> 8,193 tokens of context) while the number of split rows and of splits grows
+   within a job and from job to job; a system prompt longer than 4,096 tokens (every row split);
    greedy tokens against the CPU oracle; truncation past the window.
 4. Real size: qwen-3-4b (~30k-token row) and llama-3.1-8b (~20k) against the replay, and
    `Sutro.infer` with default engine options serving a 20k-token row untruncated.
@@ -243,6 +245,73 @@ def test_engine_long_rows_match_replay(name):
                 seed=5)
         compare(eng, rows, f"{name} schema", rep, system_prompt=synth.README_SYSTEM_PROMPT,
                 json_schema=Sentiment.model_json_schema(), max_new_tokens=16)
+    finally:
+        eng.close()
+
+
+def exact_row(ref, tpl, n_prompt, seed):
+    """A row of prose whose rendered prompt (prefix | row | suffix) is exactly n_prompt tokens."""
+    n_body = n_prompt - len(ref.encode_pieces(tpl.prefix)) - len(ref.encode_pieces(tpl.suffix))
+    text = long_text(ref, n_body + 300, seed)
+    assert len(ref.encode(text)) > n_body
+    lo, hi = 0, len(text)
+    while lo < hi:                          # the shortest cut with at least n_body tokens
+        mid = (lo + hi) // 2
+        if len(ref.encode(text[:mid])) >= n_body:
+            hi = mid
+        else:
+            lo = mid + 1
+    for c in range(max(0, lo - 8), lo + 64):
+        if len(ref.encode(text[:c])) == n_body:
+            assert len(ref.render(tpl, text[:c])) == n_prompt
+            return text[:c]
+    raise AssertionError(f"no cut of the text renders to {n_prompt} tokens")
+
+
+def split_schedule(reps):
+    """Per decode step, (rows attended in splits, most splits of a row), when every row decodes
+    from its first step on; a row's context in decode step t is prompt + 1 + t."""
+    out = []
+    for t in range(max(r.decode_steps for r in reps)):
+        ctx = [r.prompt_len + 1 + t for r in reps if t < r.decode_steps]
+        n = [-(-c // SPLIT) for c in ctx]
+        out.append((sum(k > 1 for k in n), max(n)))
+    return out
+
+
+def test_engine_rows_cross_a_split_during_decode():
+    """Rows whose context crosses 4,096 -> 4,097 in their first, second or ninth decode step, and
+    8,192 -> 8,193, beside short rows, greedy and sampled; then, on the same engine, a job with
+    fewer split rows (the grown split workspace reused) and one with more rows and splits (grown
+    again).  Every row bit-identical to its replay."""
+    eng, _ = tiny_engine("tiny-qwen3-g4")
+    try:
+        ref = RefTokenizer(eng.vocab)
+        tpl = VB.chat_template(eng.spec.family, None)
+        shorts = synth.product_reviews(3, seed=14)
+        sizes = [4095, 4096, 4088, 8190]
+        rows = [exact_row(ref, tpl, n, seed=100 + i) for i, n in enumerate(sizes)]
+        rows = [shorts[0], rows[0], rows[1], shorts[1], rows[2], rows[3]]
+        rep = Replay(eng)
+        kw = dict(max_new_tokens=16, ignore_eos=True)
+        _, reps = compare(eng, rows, "split crossing greedy", rep, **kw)
+        assert [reps[i].prompt_len for i in (1, 2, 4, 5)] == sizes
+        for i, bound in ((1, SPLIT), (2, SPLIT), (4, SPLIT), (5, 2 * SPLIT)):
+            P, steps = reps[i].prompt_len, reps[i].decode_steps
+            assert P <= bound < P + steps, (P, steps, bound)   # crossed in decode
+        sched = split_schedule(reps)
+        assert sched[0] == (2, 2) and sched[-1] == (4, 3), sched   # rows and splits both rise
+        compare(eng, rows, "split crossing sampled", rep, temperature=0.8, top_p=0.9, seed=7, **kw)
+        # fewer split rows: the workspace the first job grew is reused
+        few = [shorts[2], exact_row(ref, tpl, 4100, seed=110)]
+        _, reps = compare(eng, few, "fewer split rows", rep, **kw)
+        assert max(n for n, _ in split_schedule(reps)) == 1
+        # more split rows and more splits than the first job: it grows again
+        more = [exact_row(ref, tpl, n, seed=120 + i)
+                for i, n in enumerate((4090, 5000, 6000, 8185, 9000, 12286))] + [shorts[0]]
+        _, reps = compare(eng, more, "more split rows", rep, temperature=0.7, seed=3, **kw)
+        sched = split_schedule(reps)
+        assert sched[0] == (5, 3) and sched[-1] == (6, 4), sched
     finally:
         eng.close()
 

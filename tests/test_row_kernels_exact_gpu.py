@@ -4,8 +4,8 @@
   every in-place call) and partial last vectors, on rows whose mean squares span 2^-40 (eps
   dominates) to 2^40, plus an all-zero row.
 - The stand-alone RoPE/KV write at 12 to 64 heads per token (one to four passes of 16 heads),
-  with and without q/k-norm, Qwen and llama-scaled tables, positions up to 4095, shuffled page
-  tables and a sentinel-filled pool.
+  with and without q/k-norm, Qwen and llama-scaled tables, positions up to 32,767, shuffled
+  2,049-entry page tables and a sentinel-filled pool.
 - Embedding gathers from full-size tables, and the embedding head's L2 normalisation.
 
 Rounding follows bf16_ref: every element must equal the fp64 reference rounded at the kernel's
@@ -229,22 +229,19 @@ ROPE_HEADS = [(8, 2), (16, 8), (32, 8), (48, 8)]   # 12, 32, 48, 64 heads: 1 .. 
 @pytest.mark.parametrize("qk_norm", [True, False], ids=["qk_norm", "no_norm"])
 @pytest.mark.parametrize("hq,hkv", ROPE_HEADS)
 def test_rope_kv_write_exact(hq, hkv, qk_norm, model):
-    """Q in place and K in the pool equal the op-by-op RoPE of the (q/k-normed) heads, the dense
-    K columns equal the pool's K, V in the pool is a bit copy of the input, and pool slots no
-    token maps to keep their sentinel."""
+    """Q in place and K in the pool equal the op-by-op RoPE of the (q/k-normed) heads at
+    positions up to 32,767 (the model's 32,768-row tables, the engine's 2,049-entry page table),
+    the dense K columns equal the pool's K, V in the pool is a bit copy of the input, and pool
+    slots no token maps to keep their sentinel, as does the page every unmapped entry points at."""
     spec = MS.get_spec(model)
     nh = hq + 2 * hkv
-    T, n_slots, max_pages = 150, 3, 4096 // PAGE
-    num_pages = n_slots * max_pages + 16
+    T, n_slots, max_pages = 150, 3, KV.MAX_PAGES
     torch.manual_seed(nh * 2 + int(qk_norm) + len(model))
-    tok_slot = torch.arange(T) % n_slots
-    tok_pos = torch.empty(T, dtype=torch.long)
-    for s in range(n_slots):
-        idx = (tok_slot == s).nonzero().flatten()
-        tok_pos[idx] = torch.randperm(4096)[:len(idx)]
-    tok_pos[:2] = torch.tensor([4095, 0])
-    pt = torch.randperm(num_pages)[:n_slots * max_pages].view(n_slots, max_pages)
-    cos, sin = (t.to(DEV) for t in MS.rope_tables(spec, 4096))
+    tok_slot, tok_pos = KV.long_positions(T, n_slots, seed=nh + len(model))
+    assert set(KV.EDGE_POSITIONS) <= set(tok_pos.tolist())
+    assert (tok_pos >= 4096).float().mean() > 0.5
+    pt, num_pages, sentinel = KV.sparse_page_table(tok_slot, tok_pos, n_slots, seed=nh)
+    cos, sin = (t.to(DEV) for t in MS.rope_tables(spec, KV.MAX_POS))
     qkv = bf(torch.randn(T, nh * HD, device=DEV) * 3)
     qn = bf(torch.randn(HD, device=DEV)) if qk_norm else None
     kn = bf(torch.randn(HD, device=DEV)) if qk_norm else None
@@ -274,6 +271,7 @@ def test_rope_kv_write_exact(hq, hkv, qk_norm, model):
     written = torch.zeros(num_pages, PAGE, dtype=torch.bool, device=DEV)
     written[page, r] = True
     assert torch.all(logical.permute(0, 3, 1, 2, 4)[~written] == -3.0), "unmapped pool slots written"
+    assert not written[sentinel].any() and torch.all(logical[sentinel] == -3.0), "sentinel written"
     frac = tied_n / (T * (hq + hkv) * HD)
     print(f"[ties] rope_kv_write {hq}/{hkv} {model} qk_norm={qk_norm}: {frac:.2e} tied")
     assert frac < TIED_LIMIT

@@ -3,19 +3,24 @@
 1. Through `sb200_sample`, 512-row chunks at full vocabulary size: the penalty kernel's in-place
    logits are bit-identical to penalty_ref.apply_penalties (tests/penalty_ref.py), over
    histories that mix empty, one-token and repeat-heavy outputs, long prompts, masked and done
-   rows; the greedy token is the reference's arg-max of the penalised, masked logits; `out_tau`
-   is the reference's threshold for min_p alone and combined with top-k / top-p wherever the
-   top-p margin allows.
+   rows; the greedy token is the reference's arg-max of the penalised, masked logits, and the row
+   bookkeeping (ngen, out_tokens, out_len, done) follows it; `out_tau` is the reference's
+   threshold for min_p alone and combined with top-k / top-p wherever the top-p margin allows.
+   The same checks run at every size class of the row-history table (out_stride 1,024 to 8,192,
+   tables up to 150 KB of shared memory): hashes at their design load, probe chains that wrap
+   past the table's end, 32,000-token prompts and ids outside the vocabulary.
 2. Neutral values give the same bytes and the same launch counts as a job without them.
 3. Every row of a penalised job equals its one-row replay through the verified kernels
    (penalty_ref.PenalisedReplay over tests/engine_replay.py), bit for bit, in the engine's
-   scheduling geometries.
+   scheduling geometries, and at 2,048 to 8,192 new tokens on full-vocabulary tiny models, where
+   the engine's table needs more than 48 KiB of shared memory.
 4. A penalised row decoded alone equals the same row inside a shuffled batch.
 5. Greedy with penalties equals the CPU model (penalty_ref.generate_penalised) up to the first
    near tie.
 6. Sutro.infer, sb200_infer_text and sb200_model_infer agree on a penalised job.
 """
 import ctypes as C
+import dataclasses
 from typing import Literal
 
 import numpy as np
@@ -51,28 +56,103 @@ def dev(a, dtype=torch.int32):
 
 
 # ------------------------------------------------------------------------ 1. the sample hook
+HASH_MUL = 2654435761          # the kernel's hash: home(t) = (t * HASH_MUL) mod hash_size
+
+
+def hash_size(stride):
+    """Slots of the kernel's output-count hash: the smallest power of two >= 2 * out_stride
+    (at least 32), so live rows (at most out_stride - 1 outputs) keep its load under 0.5."""
+    h = 32
+    while h < 2 * stride:
+        h *= 2
+    return h
+
+
+def table_bytes(V, stride):
+    """Dynamic shared memory of the penalty kernel: the prompt bitmap and 8 bytes a hash slot."""
+    return (V + 31) // 32 * 4 + hash_size(stride) * 8
+
+
+def wrap_cluster(V, H, rng, n_buckets=24, per_bucket=3):
+    """Distinct tokens, per_bucket of them homed at each of the last n_buckets slots of an
+    H-slot table (t = j * HASH_MUL^-1 mod H, plus multiples of H): linear probing must carry
+    some of them past the last slot and around to slot 0."""
+    inv = pow(HASH_MUL, -1, H)
+    toks = []
+    for j in range(H - n_buckets, H):
+        base = j * inv % H
+        toks += [base + int(k) * H for k in rng.choice((V - 1 - base) // H + 1, per_bucket,
+                                                        replace=False)]
+    return np.array(toks, np.int32)
+
+
+def probes_wrap(tokens, V, H):
+    """True if some probe chain must run past the table's last slot: for some m, more distinct
+    in-range tokens are homed in the last m slots than those m slots hold (whatever the order of
+    the insertions)."""
+    t = np.unique(np.asarray(tokens, np.int64))
+    t = t[(t >= 0) & (t < V)]
+    home = (t.astype(np.uint64) * np.uint64(HASH_MUL)) % np.uint64(H)
+    from_end = np.sort((H - home).astype(np.int64))          # 1 for the last slot
+    return bool((np.arange(1, len(from_end) + 1) > from_end).any())
+
+
 class Chunk:
-    """A 512-row chunk with its prompts, histories, masks and done flags, on the GPU."""
+    """B rows (512 by default) with their prompts, histories, masks and done flags, on the GPU.
+    Row b is of kind b % 10: kinds 0-5 mix empty, one-token, repeat-heavy and stride - 1 outputs
+    (mostly repeats) with prompts of up to 3,000 tokens; 6 holds stride - 1 distinct outputs (the
+    hash at its design load); 7 a cluster homed in the table's last slots, so probes wrap to
+    slot 0, with repeats mixed in; 8 a ~32,000-token prompt that overlaps the output; 9 ids
+    outside [0, V) in the prompt and the output, which the kernel must ignore."""
+
+    KINDS = 10
 
     def __init__(self, V, seed, B=512, stride=96):
         rng = np.random.default_rng(seed)
-        self.V, self.B, self.stride = V, B, stride
+        self.V, self.B, self.stride, self.H = V, B, stride, hash_size(stride)
         self.raw = (rng.standard_normal((B, V)) * 4).astype(np.float32)
         self.pre = rng.integers(0, V, 40).astype(np.int32)
         self.suf = rng.integers(0, V, 9).astype(np.int32)
         rows, self.ngen, self.out = [], np.zeros(B, np.int32), np.zeros((B, stride), np.int32)
+        bad = np.array([-1, -7, V, V + 1, 2 ** 31 - 1, -2 ** 31], np.int64)
         for b in range(B):
             hot = rng.integers(0, V, 6)
-            kind = b % 6
-            n_row = [0, 3, 40, 3000, 200, 15][kind] + int(rng.integers(0, 8))
-            rows.append(np.where(rng.random(n_row) < 0.5, rng.choice(hot, n_row),
-                                 rng.integers(0, V, n_row)).astype(np.int32))
-            n = [0, 1, 80, 5, stride - 1, 30][kind]
-            self.out[b, :n] = np.where(rng.random(n) < 0.85, rng.choice(hot, n),
-                                       rng.integers(0, V, n))
+            kind = b % self.KINDS
+            if kind < 6:
+                n_row = [0, 3, 40, 3000, 200, 15][kind] + int(rng.integers(0, 8))
+                row = np.where(rng.random(n_row) < 0.5, rng.choice(hot, n_row),
+                               rng.integers(0, V, n_row))
+                n = [0, 1, 80, 5, stride - 1, 30][kind]
+                o = np.where(rng.random(n) < 0.85, rng.choice(hot, n), rng.integers(0, V, n))
+            elif kind == 6:
+                row = rng.integers(0, V, 20)
+                o = rng.choice(V, stride - 1, replace=False)
+            elif kind == 7:
+                cl = wrap_cluster(V, self.H, rng)
+                n = max(len(cl), min(stride - 1, 4 * len(cl)))
+                o = np.concatenate([cl, np.where(rng.random(n - len(cl)) < 0.9,
+                                                 rng.choice(cl, n - len(cl)),
+                                                 rng.integers(0, V, n - len(cl)))])
+                o = rng.permutation(o)
+                row = np.where(rng.random(100) < 0.5, rng.choice(cl, 100), rng.integers(0, V, 100))
+            elif kind == 8:
+                n = min(stride - 1, 500)
+                o = np.where(rng.random(n) < 0.6, rng.choice(hot, n), rng.integers(0, V, n))
+                n_row = 32000 - int(rng.integers(0, 50))
+                row = np.where(rng.random(n_row) < 0.3, rng.choice(o, n_row),
+                               rng.integers(0, V, n_row))
+            else:
+                n = min(stride - 1, 300)
+                o = np.where(rng.random(n) < 0.2, rng.choice(bad, n), rng.choice(hot, n))
+                row = np.where(rng.random(400) < 0.2, rng.choice(bad, 400),
+                               rng.integers(0, V, 400))
+            rows.append(np.asarray(row).astype(np.int32))
+            n = len(o)
+            self.out[b, :n] = np.asarray(o).astype(np.int32)
             self.ngen[b] = n
             # the history's own logits take +-0 and ties at the maximum
             h = np.concatenate([rows[b], self.out[b, :n]])
+            h = h[(h >= 0) & (h < V)]
             if len(h):
                 self.raw[b, h[:3]] = np.float32([0.0, -0.0, self.raw[b].max()])[:len(h[:3])]
         self.raw[:, rng.integers(0, V, 64)] = -0.0                   # -0.0 outside the histories
@@ -147,16 +227,17 @@ PEN_SETS = [dict(PEN), dict(presence_penalty=-1.0, frequency_penalty=-0.25, repe
             dict(repetition_penalty=1.7), dict(frequency_penalty=2.0)]
 
 
-@pytest.mark.parametrize("V", [151936, 128256])
-@pytest.mark.parametrize("pi", range(len(PEN_SETS)))
-def test_penalised_logits_and_greedy_token_are_exact(V, pi):
-    c, pen = chunk(V), PEN_SETS[pi]
+def check_penalised_greedy(c, pen):
+    """One greedy sb200_sample over chunk c with penalties pen: penalised logits bit-identical to
+    the reference, the reference's lowest-index arg-max drawn and booked, done rows untouched."""
     h = c.run(**pen)
     n_rewritten = 0
     for b in range(c.B):
+        n = c.ngen[b]
         if c.done[b]:
             assert (bits(h["lg"][b]) == bits(c.raw[b])).all(), b        # done rows: untouched
-            assert h["ngen"][b] == c.ngen[b]
+            assert h["ngen"][b] == n and h["len"][b] == 0 and h["done"][b] == 1, b
+            assert (h["out"][b] == c.out[b]).all(), b
             continue
         want = c.penalised(b, **pen)
         bad = np.nonzero(bits(h["lg"][b]) != bits(want))[0]
@@ -165,8 +246,55 @@ def test_penalised_logits_and_greedy_token_are_exact(V, pi):
         z = np.where(c.allowed[b], want, -np.inf)
         tok = int(np.flatnonzero(z == z.max())[0])                     # lowest index wins ties
         assert h["next"][b] == tok, (b, h["next"][b], tok)
+        # bookkeeping: the token appended after the history, the row done at out_stride tokens
+        assert h["ngen"][b] == n + 1 and h["len"][b] == n + 1, (b, h["ngen"][b], h["len"][b])
+        assert (h["out"][b, :n] == c.out[b, :n]).all() and h["out"][b, n] == tok, b
+        assert h["done"][b] == int(n + 1 >= c.stride), b
     assert n_rewritten > 0
+    return n_rewritten
+
+
+@pytest.mark.parametrize("V", [151936, 128256])
+@pytest.mark.parametrize("pi", range(len(PEN_SETS)))
+def test_penalised_logits_and_greedy_token_are_exact(V, pi):
+    c, pen = chunk(V), PEN_SETS[pi]
+    n_rewritten = check_penalised_greedy(c, pen)
     print("PENALTIES", f"V={V}", pen, f"rewritten={n_rewritten}")
+
+
+# out_stride at and around each doubling of the hash, up to the kernel's 8,192-token limit
+TABLE_STRIDES = [1024, 1025, 2048, 2049, 4096, 4097, 8192]
+_BIG = {}
+
+
+def big_chunk(V, stride):
+    """A 40-row chunk (the CPU reference stays quick at 8,192-token histories); the last one
+    built is kept for the next penalty set."""
+    if (V, stride) not in _BIG:
+        _BIG.clear()
+        _BIG[(V, stride)] = Chunk(V, seed=V + stride, B=40, stride=stride)
+    return _BIG[(V, stride)]
+
+
+@pytest.mark.parametrize("pi", [0, 1])                    # PEN_SETS[1] has the -0.0 pass
+@pytest.mark.parametrize("V", [151936, 128256])
+@pytest.mark.parametrize("stride", TABLE_STRIDES)
+def test_penalty_tables_at_every_size_class(stride, V, pi):
+    c, pen = big_chunk(V, stride), PEN_SETS[pi]
+    # the regimes: past 48 KiB the launcher opts in to more shared memory (Qwen from 1,025
+    # tokens, Llama from 2,049); hashes at their design load; probe chains that wrap; long
+    # prompts; ids outside the vocabulary, all in rows that are not done
+    tb = table_bytes(V, stride)
+    assert (tb > 48 * 1024) == (stride > (1024 if V == 151936 else 2048)), tb
+    live = [b for b in range(c.B) if not c.done[b]]
+    outs = [c.out[b, :c.ngen[b]] for b in live]
+    assert any(len(np.unique(o)) == stride - 1 for o in outs)
+    assert any(probes_wrap(o, V, c.H) for o in outs)
+    assert max(len(c.prompt(b)) for b in live) >= 32000
+    assert any(((o < 0) | (o >= V)).any() for o in outs)
+    n_rewritten = check_penalised_greedy(c, pen)
+    print("PENALTY_TABLE", f"V={V}", f"stride={stride}", f"hash={c.H}", f"smem={tb}", pen,
+          f"rewritten={n_rewritten}")
 
 
 @pytest.mark.parametrize("V", [151936, 128256])
@@ -285,6 +413,41 @@ def test_penalised_rows_match_the_replay(name, case):
     res = replay_compare(eng, rep, ROWS, f"{case}[{name}]", system_prompt=SYS, max_new_tokens=40,
                          **kw)
     assert res.stats["rows_truncated"] == 1          # the 600-word row
+
+
+def full_vocab_engine(name, window):
+    """A tiny model over its family's full-size vocabulary, with a window of `window` tokens."""
+    from sutro_b200.engine import LocalEngine
+    V = {"qwen3": 151936, "llama": 128256}[MS.get_spec(name).family]
+    spec = dataclasses.replace(MS.with_vocab(MS.get_spec(name), V), max_position=window)
+    w = MS.make_weights(spec, seed=0, std=0.05)
+    v = VB.build_vocab(spec.family, V, seed=0)
+    return LocalEngine(spec, MS.pack_for_engine(spec, w, "cuda"), v, device=0, kv_pages=2048,
+                       max_slots=4, max_prefill_tokens=1024, logit_chunk_rows=2)
+
+
+@pytest.mark.parametrize("name,max_new", [("tiny-qwen3", 2048), ("tiny-qwen3", 8192),
+                                          ("tiny-llama", 2049)])
+def test_long_penalised_jobs_match_the_replay(name, max_new):
+    """The engine sizes the table by max_new_tokens: 2,048 (the SDK's default budget) and 8,192
+    (the limit) at Qwen's vocabulary, 2,049 at Llama's, all past 48 KiB of shared memory.  Every
+    row runs its whole budget (ignore_eos), so the hash ends at its design load."""
+    eng = full_vocab_engine(name, window=max_new + 1024)
+    try:
+        tb = table_bytes(eng.spec.vocab_size, max_new)
+        assert tb > 48 * 1024, tb
+        rep = P.PenalisedReplay(eng)
+        rows = [synth.README_REVIEWS[0], synth.product_reviews(2, seed=31)[1], "ok"]
+        cases = [dict(), dict(temperature=0.8, top_k=30, top_p=0.9, seed=5, min_p=0.05)]
+        for kw in (cases if name == "tiny-qwen3" else cases[1:]):
+            res = replay_compare(eng, rep, rows, f"{name} max_new={max_new} smem={tb}",
+                                 system_prompt=SYS, max_new_tokens=max_new, ignore_eos=True,
+                                 **kw, **PEN)
+            assert all(len(t) == max_new for t in res.out_tokens)
+            assert res.stats["rows_truncated"] == 0
+    finally:
+        eng.close()
+        torch.cuda.empty_cache()
 
 
 def test_one_call_penalised_rows_match_the_replay():

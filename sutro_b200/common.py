@@ -19,7 +19,8 @@ except Exception:  # pragma: no cover - polars is absent in this image
 
 EmbeddingModelOptions = Literal["qwen-3-embedding-0.6b", "qwen-3-embedding-6b",
                                 "qwen-3-embedding-8b"]
-ModelOptions = Union[Literal["llama-3.1-8b", "qwen-3-4b", "qwen-3-0.6b", "qwen-3-embedding-0.6b"],
+ModelOptions = Union[Literal["llama-3.1-8b", "qwen-3-4b", "qwen-3-14b", "qwen-3-14b-thinking",
+                             "qwen-3-0.6b", "qwen-3-embedding-0.6b"],
                      str]
 
 

@@ -10,7 +10,9 @@
 //
 // Work item = (sequence, kv head, q tile).  A q tile packs QT = 128/G consecutive tokens x
 // the G query heads of the kv head into 128 rows (row = token*G + head), so K/V are read once
-// per GQA group and the causal frontier advances in QT-token steps.  KV is consumed in blocks
+// per GQA group and the causal frontier advances in QT-token steps.  At G = 5 that is 25 tokens
+// in 125 rows; rows 125-127 are zero padding whose outputs are never stored, and a q tile's
+// frontier can fall anywhere inside a KV block.  KV is consumed in blocks
 // of up to 128 tokens: first the prefix blocks, then the row's own blocks up to the tile's
 // diagonal.  Only the valid tokens (rounded up to 32-row TMA boxes) are loaded, and the MMAs
 // cover the same 32, 64, 96 or 128 columns: each width is its own fully unrolled path (a
@@ -56,6 +58,18 @@ constexpr int kBoxBytes = kBoxRows * 128;    // 4 KiB
 constexpr int kTcBarBytes = 256;
 constexpr int kTcSmem = 5 * kTileBytes2 + kTcBarBytes + 1024;  // Q K[2] V[2] + barriers + align
 constexpr float kRescaleThreshold = 8.0f;    // log2 units: P stays <= 2^8 before a forced rescale
+
+// The Q tile of group size G: QT = 128 / G tokens x G heads.  G * QT = 128 rows for G = 1, 2,
+// 4 and 8; at G = 5 the box {64, 5, 25} fills 125 rows and rows 125-127 are padding that no
+// TMA load writes.  Q_FULL expects exactly the bytes of the two d-half boxes.
+template <int G>
+struct QTile {
+  static constexpr int kTokens = 128 / G;
+  static constexpr int kRows = G * kTokens;
+  static constexpr uint32_t kBytes = 2u * 64u * G * kTokens * sizeof(__nv_bfloat16);
+  static_assert(kBytes == 2u * kRows * 128u && kBytes <= kTileBytes2 && kBytes % 16 == 0,
+                "the Q boxes must fill whole 128-byte rows of the Q tile");
+};
 
 struct TcGeom {
   int q_start, q_len, past, qt0, kvh;
@@ -149,6 +163,15 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
   }
   for (int i = threadIdx.x; i < 2 * kTileBytes2 / 16; i += kTcThreads)
     asm volatile("st.shared.v4.u32 [%0], {%1,%1,%1,%1};" ::"r"(s_v + 16 * i), "r"(0) : "memory");
+  if constexpr (QTile<G>::kRows < 128) {
+    // Q padding rows: zero once, so that their S / P / O rows stay finite
+    constexpr int kPad16 = (128 - QTile<G>::kRows) * 128 / 16;   // 16-byte chunks per d-half
+    for (int i = threadIdx.x; i < 2 * kPad16; i += kTcThreads) {
+      const int dh = i / kPad16;
+      const uint32_t a = s_q + dh * kHalfBytes + QTile<G>::kRows * 128 + 16 * (i - dh * kPad16);
+      asm volatile("st.shared.v4.u32 [%0], {%1,%1,%1,%1};" ::"r"(a), "r"(0) : "memory");
+    }
+  }
   fence_proxy_async_smem();   // the zeros are visible to the tensor cores' async proxy
   __syncthreads();
 
@@ -162,7 +185,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
       for (int item = blockIdx.x; item < n_items_total; item += gridDim.x, ++n) {
         const TcGeom ge = tc_geom<G>(item, hkv, items, seq_q_start, seq_q_len, seq_past);
         mbar_wait_long(bar(Q_EMPTY), (n & 1) ^ 1);
-        mbar_arrive_expect_tx(bar(Q_FULL), kTileBytes2);
+        mbar_arrive_expect_tx(bar(Q_FULL), QTile<G>::kBytes);
         tma_load_3d(s_q, &tm_q, bar(Q_FULL), 0, ge.kvh * G, ge.q_start + ge.qt0);
         tma_load_3d(s_q + kHalfBytes, &tm_q, bar(Q_FULL), 64, ge.kvh * G, ge.q_start + ge.qt0);
         for (int b = 0; b < ge.n_blocks; ++b, ++g) {
@@ -313,6 +336,10 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const float inv = 1.0f / quad_sum(l_run[h]);
+      // a padding row's t_in is QT, the first token of the next q tile, which is not ours
+      if constexpr (QTile<G>::kRows < 128) {
+        if (t_in[h] >= QTile<G>::kTokens) continue;
+      }
       const int q_own = ge.qt0 + t_in[h];
       if (q_own >= ge.q_len) continue;
       __nv_bfloat16* dst = out + static_cast<size_t>(ge.q_start + q_own) * (hq * kHeadDim) +

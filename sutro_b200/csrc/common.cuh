@@ -45,6 +45,7 @@ int dispatch_gqa(const char* who, int hq, int hkv, F&& f) {
     case 1: return f(std::integral_constant<int, 1>{});
     case 2: return f(std::integral_constant<int, 2>{});
     case 4: return f(std::integral_constant<int, 4>{});
+    case 5: return f(std::integral_constant<int, 5>{});
     case 8: return f(std::integral_constant<int, 8>{});
     default:
       set_last_error("%s: unsupported GQA group size %d", who, hq / hkv);

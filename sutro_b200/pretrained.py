@@ -10,7 +10,7 @@ same engine serves the real model:
 What is read: `config.json` (architecture → ModelSpec), `tokenizer.json` (byte-level BPE
 vocabulary, merges, special tokens), `*.safetensors` (+ `model.safetensors.index.json` when
 sharded).  Supported architectures are the ones the kernels cover: Qwen3 and Llama-3 dense
-decoders with head_dim 128 and a GQA group of 1, 2, 4 or 8.
+decoders with head_dim 128 and a GQA group of 1, 2, 4, 5 or 8.
 
 Token ids.  The GPU tokenizer starts from raw byte values, so the engine's id space has byte b
 at id b.  GPT-2-style vocabularies keep the 256 byte tokens at ids 0..255 in another order;
@@ -164,8 +164,8 @@ def spec_from_hf_config(cfg: Dict[str, Any], name: str, max_position: int = MS.C
     if head_dim != MS.HEAD_DIM:
         raise ValueError(f"head_dim {head_dim} is not supported (kernels are built for "
                          f"{MS.HEAD_DIM})")
-    if hq % hkv or hq // hkv not in (1, 2, 4, 8):
-        raise ValueError(f"GQA group {hq}/{hkv} is not supported (1, 2, 4 or 8)")
+    if hq % hkv or hq // hkv not in (1, 2, 4, 5, 8):
+        raise ValueError(f"GQA group {hq}/{hkv} is not supported (1, 2, 4, 5 or 8)")
     if cfg.get("attention_bias") or cfg.get("mlp_bias"):
         raise ValueError("projection biases are not supported")
     if cfg.get("sliding_window") and cfg.get("use_sliding_window"):

@@ -1,10 +1,11 @@
 """Kernel-level timing of the dense prefill attention (one layer) at the benchmark's shapes.
 
-    python tools/attn_bench.py [--lib PATH] [--seconds S] [--out FILE]
+    python tools/attn_bench.py [--lib PATH] [--seconds S] [--heads HQ/HKV] [--out FILE]
 
 Times sb200_attn_prefill_dense on seeded bf16 operands, qwen-3-4b heads (32 query, 8 kv heads,
-G = 4), with CUDA events over >= --seconds of work per shape after a warm-up, and prints one JSON
-line.  Shapes, one 32k-token prefill step each:
+G = 4) unless --heads says otherwise (40/8 is qwen-3-14b, G = 5), with CUDA events over
+>= --seconds of work per shape after a warm-up, and prints one JSON line.  Shapes, one
+32k-token prefill step each:
   headline   306 rows of 107 own tokens after a 46-token shared prefix (the sentiment job)
   documents  64 rows of 512 tokens, no prefix (the 512-token documents job)
 For each: ms per launch, the HBM floor (Q and K/V read once, O written once, over 3.35 TB/s),
@@ -52,8 +53,12 @@ def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", default=None)
     ap.add_argument("--seconds", type=float, default=1.0)
+    ap.add_argument("--heads", default="32/8",
+                    help="query/kv heads, e.g. 40/8 for qwen-3-14b (default: qwen-3-4b's 32/8)")
     ap.add_argument("--out", default=None, help="append the JSON line to this file as well")
     args = ap.parse_args()
+    global HQ, HKV
+    HQ, HKV = (int(x) for x in args.heads.split("/"))
     if args.lib:
         os.environ["SB200_LIB"] = os.path.abspath(args.lib)
     sys.path.insert(0, ROOT)

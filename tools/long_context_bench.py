@@ -1,9 +1,11 @@
 """Long-context timing: split-KV decode attention per layer, and one end-to-end long-document job.
 
-    python tools/long_context_bench.py [--seconds S] [--docs N] [--doc-tokens T] [--out FILE]
+    python tools/long_context_bench.py [--seconds S] [--docs N] [--doc-tokens T] [--heads HQ/HKV]
+                                       [--skip-e2e] [--out FILE]
 
-1. Decode attention, one layer, qwen-3-4b heads (32 query, 8 kv heads), through sb200_attn_decode
-   on seeded bf16 operands, CUDA events over >= --seconds of launches per shape after a warm-up:
+1. Decode attention, one layer, qwen-3-4b heads (32 query, 8 kv heads; --heads 40/8 gives
+   qwen-3-14b's), through sb200_attn_decode on seeded bf16 operands, CUDA events over
+   >= --seconds of launches per shape after a warm-up:
      12 x 32k, 24 x 16k, 48 x 8k    rows x tokens of context (about 12 GB of KV each)
      mixed       1 x 32k + 3,583 x 128, against the 3,583 short rows alone
    For each: ms per launch, the HBM floor (every row's K/V read once, over the 3.35 TB/s data
@@ -132,7 +134,8 @@ def end_to_end(args, torch) -> dict:
     kms = prof["kernel_ms"]
     # useful causal prefill attention FLOPs: 4 * 128 per (query head, visible key), every layer
     rows_tok = prof["input_tokens"] / args.docs
-    attn_flops = args.docs * 4.0 * HD * HQ * spec.n_layers * rows_tok * (rows_tok + 1) / 2
+    attn_flops = (args.docs * 4.0 * HD * spec.n_q_heads * spec.n_layers * rows_tok *
+                  (rows_tok + 1) / 2)
     res = {"docs": args.docs, "input_tokens": r.stats["input_tokens"],
            "rows_truncated": r.stats["rows_truncated"], "seconds": round(dt, 2),
            "rows_per_sec": round(args.docs / dt, 3),
@@ -152,8 +155,12 @@ def main() -> None:
     ap.add_argument("--docs", type=int, default=64)
     ap.add_argument("--doc-tokens", type=int, default=30000)
     ap.add_argument("--skip-e2e", action="store_true")
+    ap.add_argument("--heads", default="32/8",
+                    help="query/kv heads, e.g. 40/8 for qwen-3-14b (default: qwen-3-4b's 32/8)")
     ap.add_argument("--out", default=None, help="append the JSON line to this file as well")
     args = ap.parse_args()
+    global HQ, HKV
+    HQ, HKV = (int(x) for x in args.heads.split("/"))
     sys.path.insert(0, ROOT)
     import torch
     from sutro_b200 import _lib as L

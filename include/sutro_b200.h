@@ -112,6 +112,22 @@ int sb200_attn_prefill_dense(const void* qkv, int t_rows, void* out, const void*
                              int n_items, const int32_t* seq_q_start, const int32_t* seq_q_len,
                              const int32_t* seq_past, int hq, int hkv, float scale, void* stream);
 
+/* sb200_attn_prefill_dense for a row prefilled in chunks: sequence i has already prefilled its
+ * own tokens [0, seq_hist[i]) in earlier calls, and their K/V are read from the paged pool of this
+ * layer (kv_layer, page_table[seq_slot[i]], positions seq_past[i] + own index).  The qkv rows
+ * [seq_q_start[i], +seq_q_len[i]) hold its own tokens [seq_hist[i], +seq_q_len[i]).  seq_hist[i]
+ * must be a multiple of sb200_attn_prefill_hist_align(hq, hkv); then every output is bit-identical
+ * to sb200_attn_prefill_dense over the whole row.  seq_hist[i] == 0 everywhere is the dense call. */
+int sb200_attn_prefill_chunked(const void* qkv, int t_rows, void* out, const void* prefix_kv,
+                               int prefix_rows, int n_layers, int layer, const int32_t* items,
+                               int n_items, const int32_t* seq_q_start, const int32_t* seq_q_len,
+                               const int32_t* seq_past, int hq, int hkv, float scale,
+                               const void* kv_layer, const int32_t* page_table, int max_pages,
+                               const int32_t* seq_slot, const int32_t* seq_hist, void* stream);
+/* granularity of seq_hist and of the engine's prefill chunks: lcm(128, q tile) tokens
+ * (128 for GQA groups 1, 2, 4 and 8; 3,200 for 5); 0 for an unsupported group */
+int sb200_attn_prefill_hist_align(int hq, int hkv);
+
 /* K8: token-level mask of a byte DFA compiled from output_schema. */
 int sb200_fsm_build_mask(const int32_t* fsm_trans, const uint8_t* fsm_accept, int n_states,
                          const uint8_t* tok_bytes, const int32_t* tok_off, int vocab, int eos_id,

@@ -33,7 +33,7 @@ def _client() -> Sutro:
 
 def configure(**kwargs) -> Sutro:
     """(Re)create the process-wide client with constructor options — `devices`,
-    `engine_options` (max_slots, max_prefill_tokens, kv_pages, ...), `model_paths`, `verbose`,
+    `engine_options` (max_position, max_slots, max_prefill_tokens, kv_pages, ...), `model_paths`, `verbose`,
     `cache_dir`, `on_progress`, `fsm_limits` (see `Sutro.__init__`).  The reference configures its singleton
     through setters (set_api_key / set_base_url, sutro/sdk.py:58-95); a local engine's knobs
     are construction-time."""

@@ -39,6 +39,11 @@ _SIGNATURES = {
     "sb200_attn_prefill_dense": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
                                          c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                          c_int, c_float, c_void_p]),
+    "sb200_attn_prefill_chunked": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_int, c_int,
+                                           c_int, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_int, c_int, c_float, c_void_p, c_void_p, c_int,
+                                           c_void_p, c_void_p, c_void_p]),
+    "sb200_attn_prefill_hist_align": (c_int, [c_int, c_int]),
     "sb200_fsm_build_mask": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int,
                                      c_void_p, c_int, c_void_p]),
 }

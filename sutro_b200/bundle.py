@@ -3,6 +3,7 @@
 
     python -m sutro_b200.bundle --model qwen-3-4b --out /models/qwen-3-4b.sb200 [--seed 0]
     python -m sutro_b200.bundle --hf-dir /ckpt/Qwen3-4B --out /models/qwen3-4b.sb200
+    python -m sutro_b200.bundle --model qwen-3-4b --max-position 131072 --out /models/q4b-128k
 
 Layout: `manifest.json` (format 1: spec, tokenizer parameters, special-token ids, and for every
 tensor its byte offset / size in `data.bin`) + `data.bin` (bf16 weights in the engine's layout
@@ -86,15 +87,19 @@ def main():
     ap.add_argument("--model", default=None, help="named architecture, seeded random weights")
     ap.add_argument("--hf-dir", default=None, help="Hugging Face model directory (safetensors)")
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--max-position", type=int, default=None,
+                    help="context window to serve (default: the model's registered window); "
+                         "the bundle holds RoPE tables for it")
     ap.add_argument("--out", required=True)
     a = ap.parse_args()
     from .engine import LocalEngine
     if a.hf_dir:
         from .pretrained import load_pretrained
-        eng = load_pretrained(a.hf_dir, 0, kv_pages=64, max_slots=8, max_prefill_tokens=256)
+        kw = {} if a.max_position is None else {"max_position": a.max_position}
+        eng = load_pretrained(a.hf_dir, 0, kv_pages=64, max_slots=8, max_prefill_tokens=256, **kw)
     elif a.model:
         eng = LocalEngine.from_seed(a.model, seed=a.seed, device=0, kv_pages=64, max_slots=8,
-                                    max_prefill_tokens=256)
+                                    max_prefill_tokens=256, max_position=a.max_position)
     else:
         ap.error("--model or --hf-dir")
     print(export_bundle(eng, a.out))

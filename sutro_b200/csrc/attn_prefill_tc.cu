@@ -1,7 +1,9 @@
 // sutro_b200 — K3 (tensor-core path): causal varlen prefill attention on Hopper wgmma.
 //
-// The engine never splits a row's prompt over prefill steps, so a new token attends to
-// [shared prefix | the row's own new tokens].  Both live in DENSE row-major buffers here:
+// A new token attends to [shared prefix | the row's own tokens].  Both live in DENSE row-major
+// buffers here, except the own tokens of a row prefilled in chunks that earlier chunks wrote
+// (its history, attn_prefill_chunked): those are gathered from the paged pool by warps 9-11.
+// The dense sources:
 // the fused QKV epilogue (gemm_wgmma.cu) leaves post-norm / post-RoPE K and V in the qkv
 // activation buffer next to q, and the shared prefix's K/V are kept per layer in a small
 // dense side buffer.  Dense rows are what TMA wants: every operand tile below is one or a
@@ -71,16 +73,29 @@ struct QTile {
                 "the Q boxes must fill whole 128-byte rows of the Q tile");
 };
 
+// The history of a chunked prefill: each sequence's own tokens [0, hist) were prefilled by
+// earlier calls and are read from the paged KV pool (kernels.h layout) of this layer.
+struct TcHist {
+  const __nv_bfloat16* kv_layer;
+  const int32_t* page_table;
+  int max_pages;
+  const int32_t* seq_slot;
+  const int32_t* seq_hist;
+};
+
+// Own positions are counted from the row's first own token: the q tile starts at own position
+// hist + qt0, and the current call's qkv rows hold own positions [hist, hist + q_len).
 struct TcGeom {
   int q_start, q_len, past, qt0, kvh;
+  int hist, slot;
   int n_pre, n_blocks;
 };
 
-template <int G>
+template <int G, bool kHist>
 SB_DEVICE TcGeom tc_geom(int item, int hkv, const int32_t* __restrict__ items,
                          const int32_t* __restrict__ seq_q_start,
                          const int32_t* __restrict__ seq_q_len,
-                         const int32_t* __restrict__ seq_past) {
+                         const int32_t* __restrict__ seq_past, const TcHist& hs) {
   constexpr int QT = 128 / G;
   TcGeom g;
   const int w = item / hkv;
@@ -90,13 +105,16 @@ SB_DEVICE TcGeom tc_geom(int item, int hkv, const int32_t* __restrict__ items,
   g.q_start = seq_q_start[seq];
   g.q_len = seq_q_len[seq];
   g.past = seq_past[seq];
+  g.hist = kHist ? hs.seq_hist[seq] : 0;
+  g.slot = kHist ? hs.seq_slot[seq] : 0;
   g.n_pre = (g.past + kBlk - 1) / kBlk;
-  const int own_end = min(g.q_len, g.qt0 + QT);  // exclusive causal frontier of the tile
+  const int own_end = g.hist + min(g.q_len, g.qt0 + QT);  // exclusive causal frontier of the tile
   g.n_blocks = g.n_pre + (own_end + kBlk - 1) / kBlk;
   return g;
 }
 
-// block b of an item: source (prefix / own), first token, tokens the MMA covers (multiple of 16)
+// block b of an item: source (prefix / own), first token, tokens the MMA covers (multiple of 16).
+// An own block that starts below hist lies wholly in the history (hist is a multiple of kBlk).
 template <int G>
 SB_DEVICE void tc_block(const TcGeom& g, int b, bool& is_pre, int& j0, int& n16) {
   constexpr int QT = 128 / G;
@@ -107,7 +125,7 @@ SB_DEVICE void tc_block(const TcGeom& g, int b, bool& is_pre, int& j0, int& n16)
     limit = g.past - j0;
   } else {
     j0 = (b - g.n_pre) * kBlk;
-    limit = min(g.q_len, g.qt0 + QT) - j0;
+    limit = g.hist + min(g.q_len, g.qt0 + QT) - j0;
   }
   limit = min(limit, kBlk);
   n16 = (limit + 15) & ~15;
@@ -128,7 +146,7 @@ SB_DEVICE float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-template <int G>
+template <int G, bool kHist>
 __global__ void __launch_bounds__(kTcThreads, 1)
 attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, head, token) over qkv
                        const __grid_constant__ CUtensorMap tm_kv,   // 2-D (col, token) over qkv
@@ -136,7 +154,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
                        __nv_bfloat16* __restrict__ out, const int32_t* __restrict__ items,
                        int n_items_total, const int32_t* __restrict__ seq_q_start,
                        const int32_t* __restrict__ seq_q_len, const int32_t* __restrict__ seq_past,
-                       int hq, int hkv, int layer, float scale_log2) {
+                       int hq, int hkv, int layer, float scale_log2, const TcHist hs) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>(
       (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
@@ -144,7 +162,9 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
   const uint32_t s_k = s_q + kTileBytes2;                    // 2 x 32 KiB
   const uint32_t s_v = s_k + 2 * kTileBytes2;                // 2 x 32 KiB
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 5 * kTileBytes2);
-  enum { Q_FULL = 0, Q_EMPTY = 1, K_FULL = 2, K_EMPTY = 4, V_FULL = 6, V_EMPTY = 8, N_BARS = 10 };
+  // H_GO: warp 8 hands a history block's freed stage to the gather warps (chunked prefill)
+  enum { Q_FULL = 0, Q_EMPTY = 1, K_FULL = 2, K_EMPTY = 4, V_FULL = 6, V_EMPTY = 8, N_BARS = 10,
+         H_GO = 10 };
   auto bar = [&](int i) { return smem_u32(&bars[i]); };
 
   const int warp = threadIdx.x >> 5;
@@ -158,6 +178,10 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
       const bool from_consumers = i == Q_EMPTY || (i >= K_EMPTY && i < K_EMPTY + 2) ||
                                   (i >= V_EMPTY && i < V_EMPTY + 2);
       mbar_init(bar(i), from_consumers ? 8 : 1);  // consumer side: one arrival per warp
+    }
+    if constexpr (kHist) {
+      mbar_init(bar(H_GO), 1);
+      mbar_init(bar(H_GO + 1), 1);
     }
     fence_mbar_init();
   }
@@ -183,7 +207,8 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
       uint32_t g = 0;  // global block counter of this CTA
       uint32_t n = 0;  // item counter of this CTA
       for (int item = blockIdx.x; item < n_items_total; item += gridDim.x, ++n) {
-        const TcGeom ge = tc_geom<G>(item, hkv, items, seq_q_start, seq_q_len, seq_past);
+        const TcGeom ge =
+            tc_geom<G, kHist>(item, hkv, items, seq_q_start, seq_q_len, seq_past, hs);
         mbar_wait_long(bar(Q_EMPTY), (n & 1) ^ 1);
         mbar_arrive_expect_tx(bar(Q_FULL), QTile<G>::kBytes);
         tma_load_3d(s_q, &tm_q, bar(Q_FULL), 0, ge.kvh * G, ge.q_start + ge.qt0);
@@ -192,10 +217,20 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
           bool is_pre;
           int j0, n16;
           tc_block<G>(ge, b, is_pre, j0, n16);
-          const int n32 = (n16 + kBoxRows - 1) / kBoxRows;
           const uint32_t st = g & 1, ph = ((g >> 1) & 1) ^ 1;
+          if (kHist && !is_pre && j0 < ge.hist) {
+            // warps 9-11 gather this block once its stage is free.  Only this thread waits on
+            // the EMPTY barriers, for every block in order, so no wait is ever two phases behind
+            // or ahead; H_GO cannot be lapped either, since its next arrival on this stage needs
+            // this block consumed, hence gathered.
+            mbar_wait_long(bar(K_EMPTY + st), ph);
+            mbar_wait_long(bar(V_EMPTY + st), ph);
+            mbar_arrive(bar(H_GO + st));
+            continue;
+          }
+          const int n32 = (n16 + kBoxRows - 1) / kBoxRows;
           const int kcol = is_pre ? ge.kvh * kHeadDim : (hq + ge.kvh) * kHeadDim;
-          const int row0 = is_pre ? j0 : ge.q_start + j0;
+          const int row0 = is_pre ? j0 : ge.q_start + j0 - ge.hist;
 #pragma unroll
           for (int v_flow = 0; v_flow < 2; ++v_flow) {
             const int col = v_flow ? kcol + hkv * kHeadDim : kcol;
@@ -213,6 +248,48 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
                   tma_load_2d(dst, &tm_kv, full, col + dh * 64, row0 + i * kBoxRows);
               }
             }
+          }
+        }
+      }
+    } else if (kHist && warp > 8) {
+      // History blocks: 128 pool rows from 8 pages, 16-byte cp.async copies, each started when
+      // warp 8 signals that the block's stage is free (H_GO).  Own token j sits at
+      // position past + j; its pool row r = pos % 16 keeps chunk c at c ^ (r & 7), and its tile row
+      // i = j - j0 wants chunk c & 7 of d-half c >> 3 at (c & 7) ^ (i & 7) (SWIZZLE_128B).  The two
+      // XORs differ whenever past % 8 != 0, so every chunk is re-swizzled.  One thread per 96
+      // completes the stage's FULL phase after all copies have landed and been fenced to the async
+      // proxy; warp 8 skips these blocks, so each phase still has exactly one arrival.
+      const int tid = threadIdx.x - 9 * 32;
+      uint32_t g = 0, go_par = 0;  // bit st: parity of the next H_GO phase of stage st
+      for (int item = blockIdx.x; item < n_items_total; item += gridDim.x) {
+        const TcGeom ge =
+            tc_geom<G, kHist>(item, hkv, items, seq_q_start, seq_q_len, seq_past, hs);
+        for (int b = 0; b < ge.n_blocks; ++b, ++g) {
+          bool is_pre;
+          int j0, n16;
+          tc_block<G>(ge, b, is_pre, j0, n16);
+          if (is_pre || j0 >= ge.hist) continue;
+          const uint32_t st = g & 1;
+          mbar_wait_long(bar(H_GO + st), (go_par >> st) & 1);
+          go_par ^= 1u << st;
+          const int32_t* pt = hs.page_table + static_cast<size_t>(ge.slot) * hs.max_pages;
+          for (int v_flow = 0; v_flow < 2; ++v_flow) {
+            const uint32_t base = (v_flow ? s_v : s_k) + st * kTileBytes2;
+            for (int idx = tid; idx < kBlk * 16; idx += 3 * 32) {
+              const int i = idx >> 4, c = idx & 15;
+              const int pos = ge.past + j0 + i;
+              const int r = pos % kPageTokens;
+              const __nv_bfloat16* src =
+                  hs.kv_layer + kv_tile_offset(pt[pos / kPageTokens], hkv, ge.kvh, v_flow == 0) +
+                  r * kHeadDim + kv_chunk(r, c) * 8;
+              cp_async_16(base + (c >> 3) * kHalfBytes + i * 128 + (((c & 7) ^ (i & 7)) << 4), src,
+                          true);
+            }
+            cp_async_commit();
+            cp_async_wait<0>();
+            fence_proxy_async_smem();
+            named_bar_sync(1, 3 * 32);
+            if (tid == 0) mbar_arrive(bar((v_flow ? V_FULL : K_FULL) + st));
           }
         }
       }
@@ -234,7 +311,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
   }
   uint32_t g = 0, n = 0;
   for (int item = blockIdx.x; item < n_items_total; item += gridDim.x, ++n) {
-    const TcGeom ge = tc_geom<G>(item, hkv, items, seq_q_start, seq_q_len, seq_past);
+    const TcGeom ge = tc_geom<G, kHist>(item, hkv, items, seq_q_start, seq_q_len, seq_past, hs);
     float o[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) o[i] = 0.f;
@@ -275,7 +352,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q,    // 3-D (d, h
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           // columns c of this block are valid for this row iff c < vlim
-          const int vlim = min(is_pre ? ge.past - j0 : ge.qt0 + t_in[h] - j0 + 1, n16);
+          const int vlim = min(is_pre ? ge.past - j0 : ge.hist + ge.qt0 + t_in[h] - j0 + 1, n16);
           float mx = -INFINITY;
 #pragma unroll
           for (int j = 0; j < W / 8; ++j)
@@ -426,17 +503,17 @@ int tc_num_sms() {
   return n > 0 ? n : 1;
 }
 
-template <int G>
+template <int G, bool kHist>
 int launch_tc(const TcMaps& m, void* out, const int32_t* items, int n_items, const int32_t* qs,
               const int32_t* ql, const int32_t* past, int hq, int hkv, int layer, float scale,
-              cudaStream_t stream) {
-  auto kern = attn_prefill_tc_kernel<G>;
+              const TcHist& hs, cudaStream_t stream) {
+  auto kern = attn_prefill_tc_kernel<G, kHist>;
   SB_SET_MAX_SMEM(kern, kTcSmem);
   const int total = n_items * hkv;
   const int grid = std::min(total, tc_num_sms());
   kern<<<grid, kTcThreads, kTcSmem, stream>>>(m.q, m.kv, m.pre, static_cast<__nv_bfloat16*>(out),
                                               items, total, qs, ql, past, hq, hkv, layer,
-                                              scale * 1.4426950408889634f);
+                                              scale * 1.4426950408889634f, hs);
   SB_CUDA_CHECK(cudaGetLastError());
   return 0;
 }
@@ -458,9 +535,48 @@ int attn_prefill_dense(const void* qkv, int t_rows, void* out, const void* prefi
   return dispatch_gqa("attn_prefill_dense", hq, hkv, [&](auto g) {
     TcMaps m;
     if (tc_maps(TcKey{qkv, prefix_kv, t_rows, hq, hkv, prefix_rows, n_layers}, &m)) return -1;
-    return launch_tc<g.value>(m, out, items, n_items, seq_q_start, seq_q_len, seq_past, hq, hkv,
-                              prefix_kv ? layer : 0, scale, stream);
+    return launch_tc<g.value, false>(m, out, items, n_items, seq_q_start, seq_q_len, seq_past,
+                                     hq, hkv, prefix_kv ? layer : 0, scale, TcHist{}, stream);
   });
+}
+
+int attn_prefill_chunked(const void* qkv, int t_rows, void* out, const void* prefix_kv,
+                         int prefix_rows, int n_layers, int layer, const int32_t* items,
+                         int n_items, const int32_t* seq_q_start, const int32_t* seq_q_len,
+                         const int32_t* seq_past, int hq, int hkv, float scale,
+                         const void* kv_layer, const int32_t* page_table, int max_pages,
+                         const int32_t* seq_slot, const int32_t* seq_hist, cudaStream_t stream) {
+  if (n_items <= 0) return 0;
+  if (layer < 0 || layer >= std::max(n_layers, 1)) {
+    set_last_error("attn_prefill_chunked: layer %d out of range", layer);
+    return -1;
+  }
+  if (!kv_layer || !page_table || max_pages <= 0 || !seq_slot || !seq_hist) {
+    set_last_error("attn_prefill_chunked: the KV pool, page table and history arrays are required");
+    return -1;
+  }
+  const TcHist hs{static_cast<const __nv_bfloat16*>(kv_layer), page_table, max_pages, seq_slot,
+                  seq_hist};
+  return dispatch_gqa("attn_prefill_chunked", hq, hkv, [&](auto g) {
+    TcMaps m;
+    if (tc_maps(TcKey{qkv, prefix_kv, t_rows, hq, hkv, prefix_rows, n_layers}, &m)) return -1;
+    return launch_tc<g.value, true>(m, out, items, n_items, seq_q_start, seq_q_len, seq_past, hq,
+                                    hkv, prefix_kv ? layer : 0, scale, hs, stream);
+  });
+}
+
+int attn_prefill_hist_align(int hq, int hkv) {
+  if (hkv <= 0 || hq % hkv != 0) return 0;
+  const int G = hq / hkv;
+  if (G != 1 && G != 2 && G != 4 && G != 5 && G != 8) return 0;  // the groups dispatch_gqa serves
+  const int qt = attn_prefill_q_tile(hq, hkv);
+  int a = kBlk, b = qt;
+  while (b) {
+    const int t = a % b;
+    a = b;
+    b = t;
+  }
+  return kBlk / a * qt;
 }
 
 }  // namespace sb

@@ -131,6 +131,19 @@ int sb200_attn_prefill_dense(const void* qkv, int t_rows, void* out, const void*
                             STREAM(stream));
 }
 
+int sb200_attn_prefill_chunked(const void* qkv, int t_rows, void* out, const void* prefix_kv,
+                               int prefix_rows, int n_layers, int layer, const int32_t* items,
+                               int n_items, const int32_t* seq_q_start, const int32_t* seq_q_len,
+                               const int32_t* seq_past, int hq, int hkv, float scale,
+                               const void* kv_layer, const int32_t* page_table, int max_pages,
+                               const int32_t* seq_slot, const int32_t* seq_hist, void* stream) {
+  return attn_prefill_chunked(qkv, t_rows, out, prefix_kv, prefix_rows, n_layers, layer, items,
+                              n_items, seq_q_start, seq_q_len, seq_past, hq, hkv, scale, kv_layer,
+                              page_table, max_pages, seq_slot, seq_hist, STREAM(stream));
+}
+
+int sb200_attn_prefill_hist_align(int hq, int hkv) { return attn_prefill_hist_align(hq, hkv); }
+
 int sb200_fsm_build_mask(const int32_t* fsm_trans, const uint8_t* fsm_accept, int n_states,
                          const uint8_t* tok_bytes, const int32_t* tok_off, int vocab, int eos_id,
                          uint32_t* mask_bits, int mask_words, void* stream) {

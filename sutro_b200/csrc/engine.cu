@@ -29,8 +29,10 @@ namespace {
 using bf16 = __nv_bfloat16;
 
 // ---- small device helpers owned by the engine -----------------------------
-struct SeqInit {  // one admitted row
+struct SeqInit {  // one sequence of a prefill step: a row, or one chunk of a row
   int32_t slot, row, q_start, q_len, past, n_row_tok, max_new, fsm_start;
+  int32_t hist;   // own tokens prefilled by earlier chunks: this step feeds [hist, hist + q_len)
+  int32_t n_own;  // the row's own tokens in all (prompt - past); hist + q_len == n_own: last chunk
 };
 
 // Fill the flattened token batch of a prefill step from (prefix | row | suffix).
@@ -44,7 +46,7 @@ prefill_prepare_kernel(const SeqInit* __restrict__ seqs, const int32_t* __restri
   const SeqInit s = seqs[blockIdx.x];
   const int64_t roff = s.row >= 0 ? row_tok_off[s.row] : 0;
   for (int j = threadIdx.x; j < s.q_len; j += blockDim.x) {
-    const int p = s.past + j;
+    const int p = s.past + s.hist + j;
     int tok;
     if (p < n_prefix) {
       tok = prefix[p];
@@ -70,6 +72,7 @@ init_slots_kernel(const SeqInit* __restrict__ seqs, const int32_t* __restrict__ 
                   int out_stride, float* __restrict__ slot_cum_logprob,
                   int32_t* __restrict__ slot_n_row_tok) {
   const SeqInit s = seqs[blockIdx.x];
+  if (s.hist > 0) return;  // a later chunk: its row was installed with its first chunk
   // the first pt_cols entries: every page the row reserved; nothing reads the entries past them
   for (int i = threadIdx.x; i < pt_cols; i += blockDim.x)
     page_table[static_cast<size_t>(s.slot) * max_pages + i] =
@@ -82,7 +85,7 @@ init_slots_kernel(const SeqInit* __restrict__ seqs, const int32_t* __restrict__ 
     if (s.row >= 0 && out_len != nullptr) out_len[s.row] = n_forced;
     slot_state[s.slot] = s.fsm_start;
     slot_ngen[s.slot] = s.row >= 0 ? n_forced : 0;
-    slot_pos[s.slot] = s.past + s.q_len - 1;  // sampler increments: next position = prompt length
+    slot_pos[s.slot] = s.past + s.n_own - 1;  // sampler increments: next position = prompt length
     slot_done[s.slot] = 0;
     slot_row[s.slot] = s.row;
     slot_maxnew[s.slot] = s.max_new;
@@ -184,10 +187,10 @@ struct StageLayout {
     SeqInit* seqs;  // [n_seqs]
     int32_t* pt;    // [n_seqs][pt_cols] page-table rows: the pages the rows reserved
     int32_t* work;  // [n_work][2] {sequence, first query token}: dense prefill attention items
-    int32_t *slot, *q_start, *q_len, *past;  // [n_seqs] each: that attention's sequence arrays
+    int32_t *slot, *q_start, *q_len, *past, *hist;  // [n_seqs] each: that attention's arrays
     int32_t* copy;  // [n_seqs] page to seed with the shared prefix's partial last page, or -1
   };
-  size_t pt, work, slot, q_start, q_len, past, copy, words;  // offsets, and the total
+  size_t pt, work, slot, q_start, q_len, past, hist, copy, words;  // offsets, and the total
 
   StageLayout(size_t n_seqs, size_t n_work, size_t pt_cols)
       : pt(n_seqs * (sizeof(SeqInit) / 4)),
@@ -196,21 +199,26 @@ struct StageLayout {
         q_start(slot + n_seqs),
         q_len(q_start + n_seqs),
         past(q_len + n_seqs),
-        copy(past + n_seqs),
+        hist(past + n_seqs),
+        copy(hist + n_seqs),
         words(copy + n_seqs) {}
   View at(int32_t* base) const {
-    return {reinterpret_cast<SeqInit*>(base), base + pt,    base + work, base + slot,
-            base + q_start,                   base + q_len, base + past, base + copy};
+    return {reinterpret_cast<SeqInit*>(base), base + pt,   base + work,
+            base + slot,                      base + q_start, base + q_len,
+            base + past,                      base + hist, base + copy};
   }
 };
 static_assert(sizeof(SeqInit) % 4 == 0, "SeqInit records are staged as int32 words");
 
-// What forward() needs of a prefill step (device pointers into the staging buffer).
+// What forward() needs of a prefill step (device pointers into the staging buffer).  The first
+// n_final sequences end their prompt in this step, and their work items come first; a sequence
+// after them is a row's non-final chunk, which needs no last-layer attention or O/MLP.
 struct PrefillStep {
-  const int32_t* work;  // work items of the dense prefill attention
-  int n_work;
-  int n_seqs;
-  const int32_t *q_start, *q_len, *past;  // per sequence
+  const int32_t* work;  // work items of the prefill attention
+  int n_work, n_work_final;
+  int n_seqs, n_final;
+  const int32_t *slot, *q_start, *q_len, *past;  // per sequence
+  const int32_t* hist;  // per sequence, or nullptr when no sequence has history in the pool
   bool keep_prefix;  // this pass is the shared prefix's: keep its K/V in prefix_kv
 };
 
@@ -229,6 +237,7 @@ struct Engine {
   std::vector<const void*> ln1, ln2, wqkv, wo, wgu, wd, qn, kn;
   cudaStream_t stream = nullptr;
   int qkv_dim = 0, q_dim = 0, max_pages = 0, t_max = 0, logit_rows = 0, q_tile = 0;
+  int chunk_tokens = 0;  // prefill chunk of a row longer than max_prefill_tokens (0: none fits)
   int64_t num_pages = 0;
   size_t layer_stride = 0;  // elements between consecutive layers in the KV pool
 
@@ -284,6 +293,8 @@ struct Engine {
       set_last_error("engine_create: GQA group %d is too large", c.n_q_heads / c.n_kv_heads);
       return -1;
     }
+    const int align = attn_prefill_hist_align(c.n_q_heads, c.n_kv_heads);
+    chunk_tokens = align > 0 ? c.max_prefill_tokens / align * align : 0;
     num_pages = c.num_pages;
     layer_stride = num_pages * kv_page_elems(c.n_kv_heads);
     SB_CUDA_CHECK(cudaGetDevice(&device));
@@ -377,10 +388,18 @@ struct Engine {
                                         cols * sizeof(bf16), T, cudaMemcpyDeviceToDevice, stream));
       }
       if (pf) {
-        SB_K(SB200_KC_ATTN_PREFILL,
-             attn_prefill_dense(qkv, t_max, attn, prefix_kv, prefix_rows, c.n_layers, l, pf->work,
-                                pf->n_work, pf->q_start, pf->q_len, pf->past, c.n_q_heads,
-                                c.n_kv_heads, scale, stream));
+        const int nw = l + 1 < c.n_layers ? pf->n_work : pf->n_work_final;
+        if (nw > 0 && !pf->hist)
+          SB_K(SB200_KC_ATTN_PREFILL,
+               attn_prefill_dense(qkv, t_max, attn, prefix_kv, prefix_rows, c.n_layers, l,
+                                  pf->work, nw, pf->q_start, pf->q_len, pf->past, c.n_q_heads,
+                                  c.n_kv_heads, scale, stream));
+        else if (nw > 0)
+          SB_K(SB200_KC_ATTN_PREFILL,
+               attn_prefill_chunked(qkv, t_max, attn, prefix_kv, prefix_rows, c.n_layers, l,
+                                    pf->work, nw, pf->q_start, pf->q_len, pf->past, c.n_q_heads,
+                                    c.n_kv_heads, scale, kv_layer(l), page_table, max_pages,
+                                    pf->slot, pf->hist, stream));
       } else {
         SB_K(SB200_KC_ATTN_DECODE,
              attn_decode(qkv, attn, kv_layer(l), page_table, max_pages, row_slot, ctx_len, T,
@@ -390,10 +409,10 @@ struct Engine {
       }
       if (!pf || l + 1 < c.n_layers) {
         if (layer_tail(l, attn, t_max, x, x, T)) return -1;
-      } else if (!pf->keep_prefix) {
+      } else if (!pf->keep_prefix && pf->n_final > 0) {
         // last tokens: attention rows -> the dead qkv buffer (wider than attn: they fit),
         // residual rows -> hl; the down GEMM writes the result to rows [0, n) of x
-        const int n = pf->n_seqs;
+        const int n = pf->n_final;
         SB_K(SB200_KC_EMBED, gather_rows(last_idx, attn, qkv, n, q_dim, stream));
         SB_K(SB200_KC_EMBED, gather_rows(last_idx, x, hl, n, c.d_model, stream));
         if (layer_tail(l, qkv, n, hl, x, n)) return -1;
@@ -591,6 +610,8 @@ struct JobRun {
   std::vector<int32_t> active;    // slots in the decode batch
   std::vector<int32_t> slot_ctx;  // host mirror: position of the next fed token
   std::vector<SeqInit> batch;     // the sequences of the next prefill step
+  SeqInit chunked{};              // the row being prefilled in chunks (slot -1: none); its hist
+                                  // is the first own token of its next chunk
   int prefix_tail_page = -1;      // physical page holding the partial tail of the shared prefix
   int64_t next_row = 0, rows_done = 0, in_tokens = 0, prefill_tokens = 0, decode_tokens = 0;
   int64_t steps_prefill = 0, steps_decode = 0;
@@ -600,6 +621,7 @@ struct JobRun {
       : e(engine), job(j), p(std::move(spec)), S(engine.cfg.max_slots), slot_pages(S + 1),
         slot_ctx(S, 0) {
     for (int s = S - 1; s >= 0; --s) free_slots.push_back(s);
+    chunked.slot = -1;
   }
   ~JobRun() {
     for (const auto& v : slot_pages) e.free_pages.insert(e.free_pages.end(), v.begin(), v.end());
@@ -628,7 +650,7 @@ struct JobRun {
       e.prefix_rows = n;
       cudaMemsetAsync(e.prefix_kv, 0, elems * sizeof(bf16), e.stream);
     }
-    batch.assign(1, SeqInit{S, -1, 0, n, 0, 0, 1, -1});
+    batch.assign(1, SeqInit{S, -1, 0, n, 0, 0, 1, -1, 0, n});
     if (prefill(n, true)) return -1;
     if (n % kPageTokens != 0) prefix_tail_page = pages.back();
     prefill_tokens = n;
@@ -637,12 +659,30 @@ struct JobRun {
   }
 
   // Takes rows in order while a slot, the prefill budget and the KV pool allow, reserves each
-  // row's pages up front and runs their prefill step.  Returns the rows admitted, or -1.
+  // row's pages up front and runs their prefill step.  A row whose new tokens exceed the budget is
+  // prefilled in chunks of e.chunk_tokens, one row at a time: each step carries its next chunk
+  // first, and new rows fill the rest of the budget.  Returns the sequences prefilled, or -1.
   int admit() {
     const auto& c = e.cfg;
     batch.clear();
     int T = 0;
-    while (next_row < job.n_rows && !free_slots.empty() && static_cast<int>(batch.size()) < S) {
+    SeqInit held{};  // the in-flight row's next chunk, when it is not its last
+    held.slot = -1;
+    if (chunked.slot >= 0) {
+      SeqInit x = chunked;
+      x.q_start = 0;
+      x.q_len = std::min(e.chunk_tokens, x.n_own - x.hist);
+      T = x.q_len;
+      if (x.hist + x.q_len == x.n_own) {
+        batch.push_back(x);
+        chunked.slot = -1;
+      } else {
+        held = x;
+        chunked.hist += x.q_len;
+      }
+    }
+    while (next_row < job.n_rows && !free_slots.empty() &&
+           static_cast<int>(batch.size()) + (held.slot >= 0) < S) {
       const int64_t r = next_row;
       const int P = p.n_prefix + p.n_row_tok[r] + p.n_suffix;
       if (P <= 0) {
@@ -653,18 +693,21 @@ struct JobRun {
       // the prompt ends inside the prefix
       if (past < p.prefix_cached) past = (past / kPageTokens) * kPageTokens;
       const int q_len = P - past;
-      if (T + q_len > c.max_prefill_tokens) {
-        if (batch.empty()) {
-          set_last_error("engine: row %lld needs %d prefill tokens > max_prefill_tokens=%d",
-                         (long long)r, q_len, c.max_prefill_tokens);
-          return -1;
-        }
-        break;
+      const bool chunks = q_len > c.max_prefill_tokens;
+      if (chunks && e.chunk_tokens <= 0) {
+        set_last_error("engine: row %lld needs %d prefill tokens > max_prefill_tokens=%d, and "
+                       "longer rows are prefilled in chunks of a multiple of %d tokens",
+                       (long long)r, q_len, c.max_prefill_tokens,
+                       attn_prefill_hist_align(c.n_q_heads, c.n_kv_heads));
+        return -1;
       }
+      const int first = chunks ? e.chunk_tokens : q_len;
+      if (T + first > c.max_prefill_tokens || (chunks && (held.slot >= 0 || chunked.slot >= 0)))
+        break;
       const int total_pages = (P + p.max_new + kPageTokens - 1) / kPageTokens;
       const int own = total_pages - past / kPageTokens;
       if (static_cast<int64_t>(e.free_pages.size()) < own) {
-        if (batch.empty() && active.empty()) {
+        if (batch.empty() && active.empty() && held.slot < 0) {
           set_last_error("engine: KV pool (%lld pages) cannot hold one row of %d tokens",
                          (long long)e.num_pages, P + p.max_new);
           return -1;
@@ -677,20 +720,31 @@ struct JobRun {
         slot_pages[slot].push_back(e.free_pages.back());
         e.free_pages.pop_back();
       }
-      batch.push_back(SeqInit{slot, static_cast<int32_t>(r), T, q_len, past, p.n_row_tok[r],
-                              p.max_new, p.has_fsm ? job.fsm_start : -1});
+      const SeqInit x{slot, static_cast<int32_t>(r), T, first, past, p.n_row_tok[r],
+                      p.max_new, p.has_fsm ? job.fsm_start : -1, 0, q_len};
       slot_ctx[slot] = P;
-      T += q_len;
+      T += first;
       in_tokens += P;
       ++next_row;
+      if (chunks) {
+        held = x;
+        chunked = x;
+        chunked.hist = first;
+        break;  // the non-final chunk is the step's last sequence
+      }
+      batch.push_back(x);
     }
+    if (held.slot >= 0) batch.push_back(held);
     if (batch.empty()) return 0;
     if (prefill(T, false)) return -1;
     prefill_tokens += T;
     ++steps_prefill;
-    for (const SeqInit& s : batch) active.push_back(s.slot);
+    for (const SeqInit& s : batch)
+      if (s.hist + s.q_len == s.n_own) active.push_back(s.slot);
     return static_cast<int>(batch.size());
   }
+
+  bool chunking() const { return chunked.slot >= 0; }
 
   // One prefill step over the sequences in `batch`, T new tokens in all: stages and uploads
   // them, installs their page-table rows and decode state, and runs the stack; then, except in
@@ -698,9 +752,15 @@ struct JobRun {
   int prefill(int T, bool prefix_pass) {
     const auto& c = e.cfg;
     const int n = static_cast<int>(batch.size());
-    int n_work = 0, pt_cols = 1;
+    int n_work = 0, n_work_final = 0, n_final = 0, pt_cols = 1;
+    bool any_hist = false;
     for (const SeqInit& s : batch) {
       n_work += (s.q_len + e.q_tile - 1) / e.q_tile;
+      if (s.hist + s.q_len == s.n_own) {  // only a step's last sequence may be a non-final chunk
+        n_work_final = n_work;
+        ++n_final;
+      }
+      any_hist |= s.hist > 0;
       const int reserved = s.past / kPageTokens + static_cast<int>(slot_pages[s.slot].size());
       pt_cols = std::max(pt_cols, reserved);
     }
@@ -719,8 +779,10 @@ struct JobRun {
       h.q_start[i] = s.q_start;
       h.q_len[i] = s.q_len;
       h.past[i] = s.past;
-      // positions [16*(past/16), past) of the first own page hold prefix tokens: seed them
-      h.copy[i] = s.past % kPageTokens != 0 ? own[0] : -1;
+      h.hist[i] = s.hist;
+      // positions [16*(past/16), past) of the first own page hold prefix tokens: seed them, with
+      // the row's first chunk (later chunks' own tokens are in that page by then)
+      h.copy[i] = s.past % kPageTokens != 0 && s.hist == 0 ? own[0] : -1;
       for (int t0 = 0; t0 < s.q_len; t0 += e.q_tile, ++wi) {
         h.work[2 * wi] = i;
         h.work[2 * wi + 1] = t0;
@@ -745,18 +807,21 @@ struct JobRun {
           e.kv_pool, e.layer_stride, kv_page_elems(c.n_kv_heads), prefix_tail_page, d.copy);
     }
     SB_CUDA_CHECK(cudaGetLastError());
-    const PrefillStep step{d.work, n_work, n, d.q_start, d.q_len, d.past, prefix_pass};
+    const PrefillStep step{d.work,    n_work, n_work_final, n,
+                           n_final,   d.slot, d.q_start,    d.q_len,
+                           d.past,    any_hist ? d.hist : nullptr, prefix_pass};
     if (e.forward(T, &step)) return -1;
-    if (prefix_pass) return 0;
+    if (prefix_pass || n_final == 0) return 0;
+    const int n_head = n_final;
     if (p.embed_mode) {
-      if (rmsnorm(e.x, e.w.final_norm, e.hn, n, c.d_model, c.rms_eps, e.stream)) return -1;
-      if (l2_normalize_rows(e.hn, e.embed_tmp, n, c.d_model, e.stream)) return -1;
-      scatter_embed_kernel<<<n, 128, 0, e.stream>>>(e.embed_tmp, d.seqs, job.out_embed_dev,
-                                                    c.d_model);
+      if (rmsnorm(e.x, e.w.final_norm, e.hn, n_head, c.d_model, c.rms_eps, e.stream)) return -1;
+      if (l2_normalize_rows(e.hn, e.embed_tmp, n_head, c.d_model, e.stream)) return -1;
+      scatter_embed_kernel<<<n_head, 128, 0, e.stream>>>(e.embed_tmp, d.seqs, job.out_embed_dev,
+                                                         c.d_model);
       SB_CUDA_CHECK(cudaGetLastError());
       return 0;
     }
-    return e.head_and_sample(n, d.slot, job, p.has_fsm, true);
+    return e.head_and_sample(n_head, d.slot, job, p.has_fsm, true);
   }
 
   // One decode step: one token for every slot in the decode batch.
@@ -869,9 +934,10 @@ int Engine::run(const sb200_job& job, sb200_job_stats* stats) {
   int rc = 0;
   while (rc == 0 && j.rows_done < N) {
     // ---- admission: refill free slots with new rows (their prefill) ----
+    // (a row being prefilled in chunks takes its next chunk after every decode step)
     const int64_t n_free = static_cast<int64_t>(j.free_slots.size());
-    if (j.next_row < N && n_free > 0 &&
-        (j.active.empty() || n_free >= min_admit || N - j.next_row <= n_free)) {
+    if (j.chunking() || (j.next_row < N && n_free > 0 &&
+                         (j.active.empty() || n_free >= min_admit || N - j.next_row <= n_free))) {
       const int n = j.admit();
       if (n < 0) {
         rc = -1;
@@ -881,7 +947,8 @@ int Engine::run(const sb200_job& job, sb200_job_stats* stats) {
         rc = j.retire();
         if (rc == 0 && job.progress)
           job.progress(j.rows_done, j.in_tokens, j.decode_tokens, job.progress_user);
-        continue;  // try to admit more before decoding
+        if (rc != 0 || !j.chunking() || j.active.empty())
+          continue;  // try to admit more before decoding
       }
     }
     if (j.active.empty()) {

@@ -122,6 +122,16 @@ int attn_prefill_dense(const void* qkv, int t_rows, void* out, const void* prefi
                        const int32_t* seq_q_start, const int32_t* seq_q_len,
                        const int32_t* seq_past, int hq, int hkv, float scale, cudaStream_t stream);
 int attn_prefill_q_tile(int hq, int hkv);  // query tokens per work item: 128 / G
+// The same attention for rows prefilled in chunks: sequence i's own tokens [0, seq_hist[i]) come
+// from the paged pool (kv_layer, page_table row seq_slot[i]); seq_hist[i] is a multiple of
+// attn_prefill_hist_align(), which makes the result bit-identical to one unchunked call.
+int attn_prefill_chunked(const void* qkv, int t_rows, void* out, const void* prefix_kv,
+                         int prefix_rows, int n_layers, int layer, const int32_t* items,
+                         int n_items, const int32_t* seq_q_start, const int32_t* seq_q_len,
+                         const int32_t* seq_past, int hq, int hkv, float scale,
+                         const void* kv_layer, const int32_t* page_table, int max_pages,
+                         const int32_t* seq_slot, const int32_t* seq_hist, cudaStream_t stream);
+int attn_prefill_hist_align(int hq, int hkv);  // lcm(128, q tile); 0 for an unsupported group
 
 // bf16 tensor map, 128-byte swizzle, rank 2..5 (gemm_wgmma.cu)
 int encode_tmap_bf16(CUtensorMap* out, const void* ptr, int rank, const uint64_t* dims,

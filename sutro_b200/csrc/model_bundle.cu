@@ -248,8 +248,10 @@ int sb200_model_open(const char* dir, int device, int max_slots, int max_prefill
     c.embedding_model = static_cast<int>(num(*spec, "embedding_model"));
     c.eos_id = static_cast<int>(num(*spec, "eos_id"));
     c.max_slots = max_slots > 0 ? max_slots : 512;
-    // a prompt is never split over prefill steps: the default step holds one full-window row
-    c.max_prefill_tokens = max_prefill_tokens > 0 ? max_prefill_tokens : std::max(8192, c.max_position);
+    // the default step holds one row of up to 32,768 tokens; longer rows are prefilled in chunks
+    c.max_prefill_tokens = max_prefill_tokens > 0
+                               ? max_prefill_tokens
+                               : std::max(8192, std::min(c.max_position, 32768));
     c.logit_chunk_rows = 1024;
     c.min_admit_rows = std::max(1, c.max_slots / 4);
     for (auto& kv : spc->o) m->specials[kv.first] = static_cast<int>(strtod(kv.second.s.c_str(), nullptr));

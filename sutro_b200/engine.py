@@ -403,9 +403,10 @@ class JobOptions:
 
 
 def default_max_prefill_tokens(spec: MS.ModelSpec) -> int:
-    """A prompt is never split over prefill steps, so the default step holds one row that fills
-    the context window, and at least 8,192 tokens."""
-    return max(8192, spec.max_position)
+    """The default step holds one row that fills a window of up to 32,768 tokens, and at least
+    8,192 tokens.  Rows of longer windows are prefilled in chunks, so activation memory stays
+    that of a 32,768-token step."""
+    return max(8192, min(spec.max_position, 32768))
 
 
 class LocalEngine:
@@ -469,9 +470,11 @@ class LocalEngine:
 
     # ---- construction helpers -------------------------------------------
     @classmethod
-    def from_seed(cls, model: str, seed: int = 0, device=0, vocab_seed: int = 0, **kw):
-        """Random-init replica of a named architecture (no checkpoints exist offline)."""
-        spec = MS.get_spec(model)
+    def from_seed(cls, model: str, seed: int = 0, device=0, vocab_seed: int = 0,
+                  max_position: Optional[int] = None, **kw):
+        """Random-init replica of a named architecture (no checkpoints exist offline), serving
+        a `max_position`-token window (None: the registered one; see `modelspec.with_window`)."""
+        spec = MS.with_window(MS.get_spec(model), max_position)
         dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device)
         if spec.n_params() > 50_000_000:
             weights = MS.make_engine_weights_on_device(spec, seed, dev)
@@ -845,8 +848,9 @@ class MultiGpuEngine:
         self.tokenizer = engines[0].tokenizer
 
     @classmethod
-    def from_seed(cls, model: str, devices: Sequence[int], seed: int = 0, vocab_seed: int = 0, **kw):
-        spec = MS.get_spec(model)
+    def from_seed(cls, model: str, devices: Sequence[int], seed: int = 0, vocab_seed: int = 0,
+                  max_position: Optional[int] = None, **kw):
+        spec = MS.with_window(MS.get_spec(model), max_position)
         devs = [torch.device("cuda", d) for d in devices]
         if spec.n_params() > 50_000_000:
             w0 = MS.make_engine_weights_on_device(spec, seed, devs[0])

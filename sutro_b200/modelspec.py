@@ -35,7 +35,8 @@ class ModelSpec:
     rope_theta: float
     qk_norm: bool
     max_position: int = 4096          # context window the engine serves (truncate_rows bound)
-    rope_scaling: Optional[dict] = None  # llama3-style {"factor","low_freq_factor",...}
+    rope_scaling: Optional[dict] = None  # llama3 {"factor","low_freq_factor",...} or yarn
+                                         # {"rope_type": "yarn", "factor", "original_max_..."}
     embedding_model: bool = False     # prefill-only, last-token pool + L2 normalise
     head_dim: int = HEAD_DIM
 
@@ -82,8 +83,8 @@ def _reg(s: ModelSpec) -> ModelSpec:
     return s
 
 
-# The real models serve 32,768-token windows: Qwen3's trained context, and for Llama-3.1 the
-# longest row one prefill step holds (a prompt is never split over prefill steps).
+# The real models serve 32,768-token windows by default: Qwen3's native context.  Longer windows
+# are opt-in (`with_window`).
 CONTEXT_WINDOW = 32768
 QWEN3_0_6B = _reg(ModelSpec("qwen-3-0.6b", "qwen3", 28, 1024, 16, 8, 3072, 151936, True, 1e-6,
                             1e6, True, max_position=CONTEXT_WINDOW))
@@ -126,13 +127,89 @@ def with_vocab(spec: ModelSpec, vocab_size: int) -> ModelSpec:
     return replace(spec, vocab_size=vocab_size)
 
 
+# Windows past the registered one, by model name: ("rope", limit) keeps the model's RoPE up to
+# `limit` positions (Llama-3.1 is trained to 131,072 with the llama3 scaling it already has);
+# "yarn" allows k x the registered window for k in YARN_FACTORS and switches the model to YaRN
+# with factor k over the registered window (Qwen3's model cards: "32,768 natively, 131,072 with
+# YaRN").  YaRN rescales every position, so it changes short rows' outputs too.  Models not
+# listed (qwen-3-0.6b, the embedding model) serve their registered window at most.  The tiny
+# test models go up to 4x theirs, so long rows can be checked at small sizes.
+YARN_FACTORS = (2, 3, 4)
+LONG_WINDOWS: Dict[str, tuple] = {
+    "llama-3.1-8b": ("rope", 131072),
+    "qwen-3-4b": ("yarn", None),
+    "qwen-3-14b": ("yarn", None),
+    "tiny-qwen3": ("yarn", None),
+    "tiny-qwen3-g4": ("yarn", None),
+    "tiny-qwen3-g5": ("yarn", None),
+    "tiny-qwen3-embedding": ("yarn", None),
+    "tiny-llama": ("rope", 4 * 512),
+}
+
+
+def with_window(spec: ModelSpec, max_position: Optional[int] = None) -> ModelSpec:
+    """`spec` serving a `max_position`-token context window (None: the registered window, the
+    spec itself).  Raises ValueError for a window the model does not support, naming its limit."""
+    if max_position is None:
+        return spec
+    w, base = int(max_position), spec.max_position
+    if w <= 0:
+        raise ValueError(f"max_position must be positive (got {max_position})")
+    if w <= base:
+        return spec if w == base else replace(spec, max_position=w)
+    kind, limit = LONG_WINDOWS.get(spec.name, (None, base))
+    if kind == "rope":
+        if w > limit:
+            raise ValueError(f"{spec.name} serves at most {limit} positions (asked {w})")
+        return replace(spec, max_position=w)
+    if kind == "yarn":
+        k = w // base
+        if w % base or k not in YARN_FACTORS:
+            allowed = ", ".join(str(f * base) for f in YARN_FACTORS)
+            raise ValueError(f"{spec.name} serves {base} positions natively and {allowed} with "
+                             f"YaRN (asked {w})")
+        return replace(spec, max_position=w, rope_scaling={
+            "rope_type": "yarn", "factor": float(k), "original_max_position_embeddings": base})
+    raise ValueError(f"{spec.name} serves at most {base} positions (asked {w})")
+
+
 # --------------------------------------------------------------------------- RoPE tables
+def _is_yarn(spec: ModelSpec) -> bool:
+    return bool(spec.rope_scaling) and spec.rope_scaling.get("rope_type") == "yarn"
+
+
+def rope_attention_factor(spec: ModelSpec) -> float:
+    """The factor YaRN applies to cos and sin: 0.1 ln(factor) + 1 (1 without YaRN)."""
+    f = float(spec.rope_scaling["factor"]) if _is_yarn(spec) else 1.0
+    return 0.1 * math.log(f) + 1.0 if f > 1 else 1.0
+
+
+def _yarn_inv_freq(spec: ModelSpec, pos_freqs: torch.Tensor) -> torch.Tensor:
+    """Inverse frequencies of a yarn rope_scaling, restating transformers 5.5.0
+    `_compute_yarn_parameters` with the defaults a Qwen3 config leaves implicit: beta_fast 32,
+    beta_slow 1 and a truncated correction range."""
+    sc, hd, base = spec.rope_scaling, spec.head_dim, spec.rope_theta
+    factor, old = float(sc["factor"]), sc["original_max_position_embeddings"]
+
+    def corr_dim(rot):
+        return hd * math.log(old / (rot * 2 * math.pi)) / (2 * math.log(base))
+    low, high = max(math.floor(corr_dim(32)), 0), min(math.ceil(corr_dim(1)), hd - 1)
+    if low == high:
+        high += 0.001
+    ramp = torch.clamp((torch.arange(hd // 2, dtype=torch.float32) - low) / (high - low), 0, 1)
+    extra = 1 - ramp
+    return (1.0 / (factor * pos_freqs)) * (1 - extra) + (1.0 / pos_freqs) * extra
+
+
 def rope_inv_freq(spec: ModelSpec) -> torch.Tensor:
     """fp32 inverse frequencies, restating transformers 5.5.0 modeling_rope_utils.py
-    (default: :130-160, llama3: :550-600)."""
+    (default: :130-160, llama3: :550-600, yarn: `_compute_yarn_parameters`)."""
     hd = spec.head_dim
-    inv = 1.0 / (spec.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.int64).float() / hd))
+    pos_freqs = spec.rope_theta ** (torch.arange(0, hd, 2, dtype=torch.int64).float() / hd)
+    inv = 1.0 / pos_freqs
     sc = spec.rope_scaling
+    if _is_yarn(spec):
+        return _yarn_inv_freq(spec, pos_freqs)
     if sc:
         factor, lo, hi = sc["factor"], sc["low_freq_factor"], sc["high_freq_factor"]
         old = sc["original_max_position_embeddings"]
@@ -147,12 +224,17 @@ def rope_inv_freq(spec: ModelSpec) -> torch.Tensor:
 
 
 def rope_tables(spec: ModelSpec, max_pos: Optional[int] = None):
-    """(cos, sin) as bf16 [max_pos, head_dim/2] — computed in fp32 then rounded to the
-    model dtype exactly as the reference model does before applying them."""
+    """(cos, sin) as bf16 [max_pos, head_dim/2] — computed in fp32 (YaRN: times its attention
+    factor, in fp32) then rounded to the model dtype exactly as the reference model does before
+    applying them."""
     n = max_pos or spec.max_position
     inv = rope_inv_freq(spec)
     freqs = torch.arange(n, dtype=torch.float32)[:, None] * inv[None, :]
-    return freqs.cos().to(torch.bfloat16), freqs.sin().to(torch.bfloat16)
+    cos, sin = freqs.cos(), freqs.sin()
+    if _is_yarn(spec):
+        att = rope_attention_factor(spec)
+        cos, sin = cos * att, sin * att
+    return cos.to(torch.bfloat16), sin.to(torch.bfloat16)
 
 
 # --------------------------------------------------------------------------- weights

@@ -25,6 +25,7 @@ from __future__ import annotations
 import glob
 import json
 import os
+from dataclasses import replace
 from typing import Any, Dict, List, Optional, Tuple
 
 import numpy as np
@@ -171,12 +172,47 @@ def spec_from_hf_config(cfg: Dict[str, Any], name: str, max_position: int = MS.C
     if cfg.get("sliding_window") and cfg.get("use_sliding_window"):
         raise ValueError("sliding-window attention is not supported")
     scaling = cfg.get("rope_scaling")
+    window = min(int(cfg.get("max_position_embeddings", max_position)), max_position)
     if scaling is not None:
         kind = scaling.get("rope_type", scaling.get("type"))
-        if kind != "llama3":
+        if kind == "yarn":
+            # Qwen3's published entry: {"rope_type": "yarn", "factor": 4.0,
+            # "original_max_position_embeddings": 32768}; its window is factor x original
+            unknown = sorted(set(scaling) - {"rope_type", "type", "factor",
+                                             "original_max_position_embeddings"})
+            if unknown:
+                raise ValueError(f"yarn rope scaling keys {unknown} are not supported")
+            if "factor" not in scaling or "original_max_position_embeddings" not in scaling:
+                raise ValueError("yarn rope scaling needs factor and "
+                                 "original_max_position_embeddings")
+            factor, old = float(scaling["factor"]), int(scaling["original_max_position_embeddings"])
+            if max_position > factor * old:
+                raise ValueError(f"{name} serves at most {int(factor * old)} positions with yarn "
+                                 f"factor {factor:g} over {old} (asked {max_position})")
+            scaling = {"rope_type": "yarn", "factor": factor,
+                       "original_max_position_embeddings": old}
+            window = max_position
+        elif kind == "llama3":
+            scaling = {k: scaling[k] for k in ("factor", "low_freq_factor", "high_freq_factor",
+                                               "original_max_position_embeddings")}
+        else:
             raise ValueError(f"rope scaling {kind!r} is not supported")
-        scaling = {k: scaling[k] for k in ("factor", "low_freq_factor", "high_freq_factor",
-                                           "original_max_position_embeddings")}
+    yarn = scaling is not None and scaling.get("rope_type") == "yarn"
+    base = name[:-len("-thinking")] if name.endswith("-thinking") else name
+    if max_position > MS.CONTEXT_WINDOW and not yarn:
+        # an opt-in long window: a registered model's rules apply over its native window
+        # (`modelspec.with_window`: YaRN for Qwen3, llama3 RoPE up to 131,072); any other model
+        # gets at most what its config.json gives
+        if base in MS.SPECS:
+            native = MS.SPECS[base].max_position
+            if window < native:
+                raise ValueError(f"{name}: config.json gives {window} positions, less than the "
+                                 f"registered model's {native} (asked {max_position})")
+            spec = spec_from_hf_config(cfg, MS.SPECS[base].name, native, embedding_model)
+            return replace(MS.with_window(spec, max_position), name=name)
+        if max_position > window:
+            raise ValueError(f"{name} serves at most {window} positions (asked {max_position}): "
+                             "its config.json gives no longer window")
     return MS.ModelSpec(
         name=name, family="qwen3" if mt == "qwen3" else "llama",
         n_layers=int(cfg["num_hidden_layers"]), d_model=d_model, n_q_heads=hq, n_kv_heads=hkv,
@@ -184,8 +220,7 @@ def spec_from_hf_config(cfg: Dict[str, Any], name: str, max_position: int = MS.C
         tied_embeddings=bool(cfg.get("tie_word_embeddings", False)),
         rms_eps=float(cfg.get("rms_norm_eps", 1e-6)), rope_theta=float(cfg.get("rope_theta", 1e4)),
         qk_norm=(mt == "qwen3"),
-        max_position=min(int(cfg.get("max_position_embeddings", max_position)), max_position),
-        rope_scaling=scaling, embedding_model=embedding_model)
+        max_position=window, rope_scaling=scaling, embedding_model=embedding_model)
 
 
 # --------------------------------------------------------------------------- safetensors
